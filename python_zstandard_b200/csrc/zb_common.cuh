@@ -4,6 +4,7 @@
 // and :41266-41290); everything else here is this project's own design.
 #pragma once
 #include <cstdint>
+#include <cstring>
 #include <cuda_runtime.h>
 
 typedef uint8_t  u8;
@@ -121,36 +122,108 @@ __device__ __forceinline__ u64 zb_rd64(const u8* p) { return (u64)zb_rd32(p) | (
 __device__ __forceinline__ int zb_hibit(u32 v) { return 31 - __clz(v); }
 
 // ---------------------------------------------------------------------------
-// Backward bit reader over an arbitrary byte range, built on ALIGNED 32-bit loads and 32-bit
-// funnel shifts.  (hi:lo) holds the next unread bits top-aligned; `avail` counts them.  The two
-// words below the window are loaded ahead (nx0, nx1) so that global-memory latency is off the
-// decode chain.  left() is the number of unread stream bits; it goes negative when the stream is
+// Asynchronous 16-byte global -> shared copies (cp.async.cg: cached in L2 only, never in L1).  The
+// CPU build of these sources copies at once.
+// ---------------------------------------------------------------------------
+__device__ __forceinline__ void zb_cp16(u8* sdst, const u8* gsrc)     // both 16-byte aligned
+{
+#ifdef __CUDA_ARCH__
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" :: "r"((u32)__cvta_generic_to_shared(sdst)), "l"(gsrc) : "memory");
+#else
+    memcpy(sdst, gsrc, 16);
+#endif
+}
+__device__ __forceinline__ void zb_cp_commit()
+{
+#ifdef __CUDA_ARCH__
+    asm volatile("cp.async.commit_group;" ::: "memory");
+#endif
+}
+template <int N> __device__ __forceinline__ void zb_cp_wait()         // all but the N most recent groups have landed
+{
+#ifdef __CUDA_ARCH__
+    asm volatile("cp.async.wait_group %0;" :: "n"(N) : "memory");
+#endif
+}
+
+// ---------------------------------------------------------------------------
+// Backward bit reader over an arbitrary byte range, built on 32-bit words and 32-bit funnel shifts.
+// (hi:lo) holds the next unread bits top-aligned; `avail` counts them; nx0, nx1 are the two words
+// below the window.  left() is the number of unread stream bits; it goes negative when the stream is
 // over-read (the reference's BIT_DStream_overflow, zstd/zstd.c:2517-2556).  Reads below the stream
 // start return the neighbouring bytes (not zeros): harmless, because left() < 0 fails the block.
+//
+// The words come from a RING of D 16-byte chunks in the lane's shared memory (chunk k -- bytes
+// [16k, 16k + 16) above the 16-byte aligned base -- in slot k mod D), which asynchronous copies keep
+// filled ahead of the decode: a refill that moves into chunk k requests chunk k + 1 - D, whose first
+// word is needed 4D - 7 refills later at the earliest (4D - 4 in steady state, less right after
+// init).  Every refill commits one copy group and, before it reads the ring, waits for all but the
+// 4D - 8 most recent groups of the thread; other readers' refills in between only add groups.  So a
+// copy has 4(D - 1) refills of decode to land in, which a 4-byte load issued one word ahead (one or
+// two sequence steps) could not get: lanes of a warp refill at different moments and the warp's
+// load scoreboard made nearly every refill wait for the latest lane's load.  The cp.async groups
+// are ordered, so the wait is for copies that are old.
+//
+// Memory: the copies read only the 16-byte aligned cover of [s, s + n), which never leaves a device
+// allocation (those are 256-byte aligned).  The ring must stay untouched while the reader lives;
+// the destructor waits for the copies still in flight.  The CPU build may pass no ring: the reader
+// then uses storage of its own.
 // ---------------------------------------------------------------------------
+#ifdef __CUDA_ARCH__
+#define ZB_RING_ARG(name) u8* name
+#else
+#define ZB_RING_ARG(name) u8* name = nullptr
+#endif
+template <int D>
 struct ZbBitR {
-    const u32* w; int widx; u32 hi, lo; int avail; u32 nx0, nx1; int skew_bits;
+    static_assert(D >= 2 && (D & (D - 1)) == 0, "ring depth: a power of two");
+    const u8* c; u8* ring; int widx; u32 hi, lo; int avail; u32 nx0, nx1; int skew_bits; int lo_c; u32 n_;
+#ifndef __CUDA_ARCH__
+    alignas(16) u8 own[16 * D];
+#endif
 
-    __device__ __forceinline__ bool init(const u8* s, u32 n) {
+    __device__ __forceinline__ u32 word(int j) const { return *(const u32*)(ring + ((u32)j & (4u * D - 1)) * 4u); }
+    __device__ __forceinline__ void fetch(int k) { zb_cp16(ring + ((u32)k & (D - 1)) * 16u, c + 16 * k); }
+    __device__ __forceinline__ ~ZbBitR() { zb_cp_wait<0>(); }
+
+    // start() requests the top D chunks; finish() waits for them and positions the reader at the end mark.
+    // Several readers start() before the first finish() so that their first copies overlap.
+    __device__ __forceinline__ bool start(const u8* s, u32 n, u8* ring_) {
         if (n == 0) return false;
-        u32 const last = s[n - 1];
+#ifdef __CUDA_ARCH__
+        ring = ring_;
+#else
+        ring = ring_ ? ring_ : own;
+#endif
+        c = (const u8*)((uintptr_t)s & ~(uintptr_t)15);
+        int const skew = (int)(s - c);
+        skew_bits = skew * 8; n_ = n;
+        int const top = (skew + (int)n - 1) >> 4;                 // chunk of the last byte
+        #pragma unroll
+        for (int q = 0; q < D; q++) if (top - q >= 0) fetch(top - q);
+        zb_cp_commit();
+        lo_c = top - D + 1 > 0 ? top - D + 1 : 0;                 // lowest chunk requested
+        return true;
+    }
+    __device__ __forceinline__ bool finish() {
+        zb_cp_wait<0>();
+        int const e = skew_bits / 8 + (int)n_ - 1;               // the last byte, relative to the aligned base
+        u32 const last = ring[(u32)e & (16u * D - 1)];
         if (last == 0) return false;
-        uintptr_t const a = (uintptr_t)s & ~(uintptr_t)3;
-        w = (const u32*)a;
-        int const skew = (int)((uintptr_t)s - a);
-        skew_bits = skew * 8;
-        int const P = (skew + (int)n - 1) * 8 + zb_hibit(last);   // bits from the aligned base up to the end mark
+        int const P = e * 8 + zb_hibit(last);                     // bits from the aligned base up to the end mark
         nx0 = nx1 = 0; lo = 0;
         if (P == 0) { hi = 0; avail = 0; widx = -1; return true; }
         int const wi = (P - 1) >> 5, k = P - wi * 32;              // k in 1..32 valid bits in the top word
-        hi = w[wi] << (32 - k); avail = k; widx = wi - 1;
-        if (widx >= 0) nx0 = w[widx];
-        if (widx >= 1) nx1 = w[widx - 1];
+        hi = word(wi) << (32 - k); avail = k; widx = wi - 1;
+        if (widx >= 0) nx0 = word(widx);
+        if (widx >= 1) nx1 = word(widx - 1);
         refill();
         return true;
     }
+    __device__ __forceinline__ bool init(const u8* s, u32 n, u8* ring_) { return start(s, n, ring_) && finish(); }
     // branch-free: lanes of a warp refill at different moments, so the body is predicated, not branched
     __device__ __forceinline__ void refill() {
+        zb_cp_wait<4 * D - 8>();
         bool const r = (avail <= 32) & (widx >= 0);                // lo is empty when r holds
         u32 const a = (u32)avail;
         u32 const add_hi = __funnelshift_rc(nx0, 0u, a);           // nx0 >> avail        (0 when avail == 32)
@@ -160,7 +233,10 @@ struct ZbBitR {
         avail += r ? 32 : 0;
         widx -= r ? 1 : 0;
         nx0 = r ? nx1 : nx0;
-        if (r && widx >= 1) nx1 = w[widx - 1];
+        if (r && widx >= 1) nx1 = word(widx - 1);
+        int const t = ((widx - 1) >> 2) + 1 - D;                   // nx1's chunk + 1 - D: its slot has been read out
+        if (t >= 0 && t < lo_c) { fetch(t); lo_c = t; }
+        zb_cp_commit();
     }
     __device__ __forceinline__ u32 peek(u32 nb) const { return __funnelshift_rc(hi, 0u, 32u - nb); }   // nb in 0..32
     __device__ __forceinline__ void skip(u32 nb) {                                                      // nb in 0..32

@@ -1571,7 +1571,12 @@ __global__ void zb_digest_dict(const u8* __restrict__ dict, u32 n, ZbDictDigest*
     const u8* p = dict + 8; const u8* const end = dict + n;
     {
         __align__(16) u8 ws[256]; u32 rank[13], log, nsym;
-        u32 const used = zb_huf_weights(ws, p, (u32)(end - p), log, nsym, rank);
+#ifdef __CUDA_ARCH__
+        __shared__ __align__(16) u8 ring[64];
+#else
+        u8* const ring = nullptr;
+#endif
+        u32 const used = zb_huf_weights(ws, p, (u32)(end - p), log, nsym, rank, ring);
         if (!used) { out->status = ZB_E_DICT_CORRUPTED; return; }
         zb_huf_fill(out->huf, ws, log, nsym, rank, 0, 0);          // the digest keeps the full table (read in place from global memory)
         out->huf_log = log; p += used;

@@ -54,7 +54,8 @@ __device__ __forceinline__ u32 zb_warp_incl_scan(u32 v, u32 lane)
 // --- Huffman weights (HUF_readStats_body).  Weights go to ws as nibbles; the weight-FSE table
 // --- (<= 64 cells, u16: sym | nb << 4 | next << 8) sits in ws + 128.
 // returns header bytes consumed (0 = error); out: log, rank[] (count of every weight)
-__device__ static u32 zb_huf_weights(u8* ws, const u8* s, u32 n, u32& out_log, u32& out_nsym, u32* rank)
+// `ring`: 64 bytes of the lane's shared memory for the bit reader (ws is full here)
+__device__ static u32 zb_huf_weights(u8* ws, const u8* s, u32 n, u32& out_log, u32& out_nsym, u32* rank, ZB_RING_ARG(ring))
 {
     u8* const wn = ws;                       // 128 bytes: 256 nibbles
     u16* const wt = (u16*)(ws + 128);        // 64 cells
@@ -101,8 +102,8 @@ __device__ static u32 zb_huf_weights(u8* ws, const u8* s, u32 n, u32& out_log, u
                 u32 const nb = log - (u32)zb_hibit(x);
                 wt[u] = (u16)(sy | (nb << 4) | (((x << nb) - size) << 8));
             }
-            ZbBitR b;
-            if (!b.init(s + 1 + used, hdr - used)) return 0;
+            ZbBitR<4> b;
+            if (!b.init(s + 1 + used, hdr - used, ring)) return 0;
             u32 s1 = b.read(log), s2 = b.read(log); b.refill();
             if (b.left() < 0) return 0;
             nsym = 0;
@@ -164,10 +165,10 @@ __device__ static void zb_huf_fill(u16* cells, const u8* ws, u32 log, u32 nsym, 
 }
 
 // one Huffman stream -> n_out bytes at out (global scratch), 4 symbols per 32-bit store where aligned
-__device__ static bool zb_huf_stream2(u8* out, u32 n_out, const u8* s, u32 n, ZbHufTab const t)
+__device__ static bool zb_huf_stream2(u8* out, u32 n_out, const u8* s, u32 n, ZbHufTab const t, u8* ring)
 {
-    ZbBitR b;
-    if (!b.init(s, n)) return false;
+    ZbBitR<4> b;
+    if (!b.init(s, n, ring)) return false;
     u32 const log = t.log;
     u32 i = 0;
     while (i < n_out && ((uintptr_t)(out + i) & 3)) { u32 v = b.peek(log); u32 c = ZB_HCELL(t, v); out[i++] = (u8)c; b.skip(c >> 8); b.refill(); }
@@ -185,7 +186,7 @@ __device__ static bool zb_huf_stream2(u8* out, u32 n_out, const u8* s, u32 n, Zb
 // The four literal streams of a block, interleaved in ONE lane: four independent bit readers advance side by
 // side, so the dependent chain of one stream (table lookup -> bit count -> shift) fills the latency slots of the
 // other three (what HUF_decompress4X1_usingDTable_internal_body does with its four BIT_DStream_t, zstd/zstd.c:39868-39964).
-struct ZbHufLane { ZbBitR b; u8* out; u32 left; };
+struct ZbHufLane { ZbBitR<4> b; u8* out; u32 left; };
 
 __device__ __forceinline__ void zb_huf_one(ZbHufLane& h, ZbHufTab const& t)
 {
@@ -199,15 +200,18 @@ __device__ __forceinline__ void zb_huf_one(ZbHufLane& h, ZbHufTab const& t)
         u32 const v3_ = h.b.peek(t.log); u32 const c3_ = ZB_HCELL(t, v3_); h.b.skip(c3_ >> 8); h.b.refill(); \
         *(u32*)h.out = (c0_ & 255) | ((c1_ & 255) << 8) | ((c2_ & 255) << 16) | (c3_ << 24); h.out += 4; h.left -= 4; } while (0)
 
-__device__ static bool zb_huf_block(u8* dstl, u32 regen, const u8* p, u32 left, bool single, ZbHufTab const t)
+// `ring`: 256 bytes of the lane's shared memory, 64 per stream for its bit reader
+__device__ static bool zb_huf_block(u8* dstl, u32 regen, const u8* p, u32 left, bool single, ZbHufTab const t, ZB_RING_ARG(ring))
 {
-    if (single) return zb_huf_stream2(dstl, regen, p, left, t);
+    if (single) return zb_huf_stream2(dstl, regen, p, left, t, ring);
     if (left < 10) return false;
     u32 const l1 = zb_rd16(p), l2 = zb_rd16(p + 2), l3 = zb_rd16(p + 4), seg = (regen + 3) / 4;
     if (6 + l1 + l2 + l3 > left || seg * 3 > regen) return false;
     u32 const l4 = left - 6 - l1 - l2 - l3;
     ZbHufLane h0, h1, h2, h3;
-    if (!h0.b.init(p + 6, l1) || !h1.b.init(p + 6 + l1, l2) || !h2.b.init(p + 6 + l1 + l2, l3) || !h3.b.init(p + 6 + l1 + l2 + l3, l4)) return false;
+    u8* const r1 = ring ? ring + 64 : nullptr; u8* const r2 = ring ? ring + 128 : nullptr; u8* const r3 = ring ? ring + 192 : nullptr;
+    if (!h0.b.start(p + 6, l1, ring) || !h1.b.start(p + 6 + l1, l2, r1) || !h2.b.start(p + 6 + l1 + l2, l3, r2) || !h3.b.start(p + 6 + l1 + l2 + l3, l4, r3)) return false;
+    if (!h0.b.finish() || !h1.b.finish() || !h2.b.finish() || !h3.b.finish()) return false;
     h0.out = dstl; h1.out = dstl + seg; h2.out = dstl + 2 * seg; h3.out = dstl + 3 * seg;
     h0.left = h1.left = h2.left = seg; h3.left = regen - 3 * seg;
     // bring every stream's output pointer to a 4-byte boundary
@@ -363,7 +367,7 @@ zb_entropy_decode(const u8* __restrict__ src, const ZbSegment* __restrict__ segs
                         hp = bs + L.hdr; hleft = L.csize;
                         if (L.type == 2) { dHuf.kind = ZB_SRC_NCOUNT; dHuf.p = hp; dHuf.n = hleft; }
                         if (dHuf.kind == ZB_SRC_NCOUNT) {
-                            u32 const used = zb_huf_weights(ws, dHuf.p, dHuf.n, hlog, hns, rank);
+                            u32 const used = zb_huf_weights(ws, dHuf.p, dHuf.n, hlog, hns, rank, tabs + lane * 64);   // no table lives in the pool during B
                             if (used == 0 || (L.type == 2 && used >= hleft)) { err = ZB_E_CORRUPTION; break; }
                             if (L.type == 2) { hp += used; hleft -= used; dHuf.n = used; }
                             wantH = true;
@@ -375,7 +379,7 @@ zb_entropy_decode(const u8* __restrict__ src, const ZbSegment* __restrict__ segs
             }
             // dictionary Huffman table: read in place from the digest (shared by every lane, cache resident)
             if (comp && B.lit_kind == ZB_LIT_SCRATCH && dHuf.kind == ZB_SRC_DICT) {
-                if (!zb_huf_block(lits + lit_i, L.regen, hp, hleft, L.single, zb_huf_full(dict.huf, dict.huf_log))) { err = ZB_E_CORRUPTION; done = true; comp = false; }
+                if (!zb_huf_block(lits + lit_i, L.regen, hp, hleft, L.single, zb_huf_full(dict.huf, dict.huf_log), ws)) { err = ZB_E_CORRUPTION; done = true; comp = false; }
             }
             ZB_EMARK(2);
             {   // claim pool space for the Huffman cells, decode; lanes that do not fit wait for the next pass
@@ -389,7 +393,7 @@ zb_entropy_decode(const u8* __restrict__ src, const ZbSegment* __restrict__ segs
                         u16* cells = (u16*)(tabs + incl - ((need + 15) & ~15u));
                         zb_huf_fill(cells, ws, hlog, hns, rank, hshift, hbase);
                         ZbHufTab t; t.cells = cells; t.log = hlog; t.shift = hshift; t.T = hT; t.base = hbase;
-                        if (!zb_huf_block(lits + lit_i, L.regen, hp, hleft, L.single, t)) { err = ZB_E_CORRUPTION; done = true; comp = false; }
+                        if (!zb_huf_block(lits + lit_i, L.regen, hp, hleft, L.single, t, ws)) { err = ZB_E_CORRUPTION; done = true; comp = false; }
                         pending = false;
                     }
                     __syncwarp();
@@ -447,8 +451,8 @@ zb_entropy_decode(const u8* __restrict__ src, const ZbSegment* __restrict__ segs
                         setup(dML, normML, msML, logML, K_ML, dict.ml, dict.ml_log, g_defML, 6, tML);
 
                         // the 3-state FSE sequence stream (restates ZSTD_decodeSequence, zstd/zstd.c:46862-46986)
-                        ZbBitR b;
-                        if (!b.init(ip, (u32)(bend - ip))) err = ZB_E_CORRUPTION;
+                        ZbBitR<8> b;                        // ring: the lane workspace (the normalized counts are consumed)
+                        if (!b.init(ip, (u32)(bend - ip), ws)) err = ZB_E_CORRUPTION;
                         else {
                             u32 sLL = b.read(tLL.log); u32 sOF = b.read(tOF.log); b.refill(); u32 sML = b.read(tML.log); b.refill();
                             const ZbFseCell* const TL = tLL.t; const ZbFseCell* const TO = tOF.t; const ZbFseCell* const TM = tML.t;
@@ -647,7 +651,7 @@ zb_entropy_blocks(const u8* __restrict__ src, const ZbBlkDesc* __restrict__ bdes
                         hp = bs + L.hdr; hleft = L.csize;
                         if (L.type == 2) { dHuf.kind = ZB_SRC_NCOUNT; dHuf.p = hp; dHuf.n = hleft; }
                         if (dHuf.kind == ZB_SRC_NCOUNT) {
-                            u32 const used = zb_huf_weights(ws, dHuf.p, dHuf.n, hlog, hns, rank);
+                            u32 const used = zb_huf_weights(ws, dHuf.p, dHuf.n, hlog, hns, rank, tabs + lane * 64);   // no table lives in the pool during B
                             if (used == 0 || (L.type == 2 && used >= hleft)) { err = ZB_E_CORRUPTION; break; }
                             if (L.type == 2) { hp += used; hleft -= used; dHuf.n = used; }
                             wantH = true;
@@ -659,7 +663,7 @@ zb_entropy_blocks(const u8* __restrict__ src, const ZbBlkDesc* __restrict__ bdes
             }
             // dictionary Huffman table: read in place from the digest (shared by every lane, cache resident)
             if (comp && B.lit_kind == ZB_LIT_SCRATCH && dHuf.kind == ZB_SRC_DICT) {
-                if (!zb_huf_block(lits + lit_i, L.regen, hp, hleft, L.single, zb_huf_full(dict.huf, dict.huf_log))) { err = ZB_E_CORRUPTION; done = true; comp = false; }
+                if (!zb_huf_block(lits + lit_i, L.regen, hp, hleft, L.single, zb_huf_full(dict.huf, dict.huf_log), ws)) { err = ZB_E_CORRUPTION; done = true; comp = false; }
             }
             ZB_EMARK(2);
             {   // claim pool space for the Huffman cells, decode; lanes that do not fit wait for the next pass
@@ -673,7 +677,7 @@ zb_entropy_blocks(const u8* __restrict__ src, const ZbBlkDesc* __restrict__ bdes
                         u16* cells = (u16*)(tabs + incl - ((need + 15) & ~15u));
                         zb_huf_fill(cells, ws, hlog, hns, rank, hshift, hbase);
                         ZbHufTab t; t.cells = cells; t.log = hlog; t.shift = hshift; t.T = hT; t.base = hbase;
-                        if (!zb_huf_block(lits + lit_i, L.regen, hp, hleft, L.single, t)) { err = ZB_E_CORRUPTION; done = true; comp = false; }
+                        if (!zb_huf_block(lits + lit_i, L.regen, hp, hleft, L.single, t, ws)) { err = ZB_E_CORRUPTION; done = true; comp = false; }
                         pending = false;
                     }
                     __syncwarp();
@@ -731,8 +735,8 @@ zb_entropy_blocks(const u8* __restrict__ src, const ZbBlkDesc* __restrict__ bdes
                         setup(dML, normML, msML, logML, K_ML, dict.ml, dict.ml_log, g_defML, 6, tML);
 
                         // the 3-state FSE sequence stream (restates ZSTD_decodeSequence, zstd/zstd.c:46862-46986)
-                        ZbBitR b;
-                        if (!b.init(ip, (u32)(bend - ip))) err = ZB_E_CORRUPTION;
+                        ZbBitR<8> b;                        // ring: the lane workspace (the normalized counts are consumed)
+                        if (!b.init(ip, (u32)(bend - ip), ws)) err = ZB_E_CORRUPTION;
                         else {
                             u32 sLL = b.read(tLL.log); u32 sOF = b.read(tOF.log); b.refill(); u32 sML = b.read(tML.log); b.refill();
                             const ZbFseCell* const TL = tLL.t; const ZbFseCell* const TO = tOF.t; const ZbFseCell* const TM = tML.t;

@@ -1,8 +1,8 @@
 """AddressSanitizer fuzz of the decode kernels' source on the CPU (tests/host_encoder.build_entropy_kernel, one emulated
 lane): mutated and truncated golden frames in exact-size heap blocks with PAD bytes of slack on both sides.
   ASAN_OPTIONS=detect_leaks=0 LD_PRELOAD=$(gcc -print-file-name=libasan.so) N=1500 SEED=7 python tools/asan_fuzz_decode.py
-Round 1: 24000 + 40000 frames with PAD=4 clean; PAD=0 shows the by-design read of the aligned 32-bit word that holds a stream's
-last byte (<= 3 bytes past the segment, inside its allocation granule on the device)."""
+The default PAD=16 covers the bit reader's by-design reads: it copies the 16-byte aligned chunks that cover a stream (up to 15
+bytes past the segment, inside its allocation granule on the device); smaller PADs show those reads."""
 import sys, os, ctypes as C, numpy as np, subprocess
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from tests import helpers, host_encoder
@@ -13,7 +13,7 @@ lib='/tmp/libzk_asan.so'
 subprocess.check_call(['g++','-std=c++17','-O1','-g','-fsanitize=address','-fno-omit-frame-pointer','-shared','-fPIC','-I/usr/local/cuda/include','-o',lib,cpp])
 L=C.CDLL(lib)
 L.t_decode_frame.argtypes=[C.c_void_p,C.c_uint64,C.c_void_p,C.c_uint32,C.c_void_p,C.c_uint64,C.POINTER(C.c_uint64),C.POINTER(C.c_uint32),C.POINTER(C.c_uint32)]
-PAD=int(os.environ.get('PAD','4'))
+PAD=int(os.environ.get('PAD','16'))
 libc=C.CDLL(None); libc.malloc.restype=C.c_void_p; libc.malloc.argtypes=[C.c_size_t]; libc.free.argtypes=[C.c_void_p]
 def decode(frame,cap,dct=b''):
     # exact-size heap blocks so that ASAN red zones sit right behind the data (+PAD slack on both sides)

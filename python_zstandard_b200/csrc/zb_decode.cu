@@ -918,6 +918,19 @@ zb_execute(const u8* __restrict__ src, const ZbFramePlace* __restrict__ place, c
 #define ZB_TILE_WARP_BYTES (2 * ZB_TILE_CAP + 64)
 #define ZB_TILE_SMEM   (ZB_TILE_WARPS * ZB_TILE_WARP_BYTES)
 
+// per-phase cycle counters of zb_execute_tile (lane 0 of every warp) exist only in tuning builds (-DZB_PHASE_TIMERS):
+// 0 frame start and literal staging, 1 literal copies, 2 frontier passes, 3 write-out
+#ifdef ZB_PHASE_TIMERS
+__device__ unsigned long long g_zb_exe_phase[4];
+#define ZB_XSTART() long long t_x = clock64(), x_acc[4] = {0, 0, 0, 0}
+#define ZB_XMARK(k) do { long long const t_ = clock64(); x_acc[k] += t_ - t_x; t_x = t_; } while (0)
+#define ZB_XFLUSH() do { if (lane == 0) for (int k_ = 0; k_ < 4; k_++) atomicAdd(&g_zb_exe_phase[k_], (unsigned long long)x_acc[k_]); } while (0)
+#else
+#define ZB_XSTART() do { } while (0)
+#define ZB_XMARK(k) do { } while (0)
+#define ZB_XFLUSH() do { } while (0)
+#endif
+
 __global__ void __launch_bounds__(ZB_TILE_WARPS * 32)
 zb_execute_tile(const u8* __restrict__ src, const ZbFramePlace* __restrict__ place, const u32* __restrict__ status,
                 const ZbBlock* __restrict__ blocks, const ZbSeq* __restrict__ seqs, const u8* __restrict__ lits,
@@ -930,6 +943,7 @@ zb_execute_tile(const u8* __restrict__ src, const ZbFramePlace* __restrict__ pla
     if (status[f] != ZB_OK) return;
     ZbFramePlace const pl = place[f];
     if (pl.dst_cap > ZB_TILE_CAP) return;                // handled by zb_execute
+    ZB_XSTART();
     u64 const blk_end = place[f + 1].blk_off;
     u32 const skew = (u32)(pl.dst_off & 15);             // same 16-byte phase in smem as in dst
     u8* const so = zb_tile + warp * ZB_TILE_WARP_BYTES + skew;          // output tile
@@ -941,8 +955,8 @@ zb_execute_tile(const u8* __restrict__ src, const ZbFramePlace* __restrict__ pla
         ZbBlock const B = blocks[bi];
         u8* const bout = so + B.out_pos;
         total = (u32)B.out_pos + B.regen;
-        if (B.kind == ZB_BLK_RAW) { const u8* p = src + B.src_pos; for (u32 i = lane; i < B.regen; i += 32) bout[i] = p[i]; __syncwarp(); continue; }
-        if (B.kind == ZB_BLK_RLE) { for (u32 i = lane; i < B.regen; i += 32) bout[i] = (u8)B.lit_byte; __syncwarp(); continue; }
+        if (B.kind == ZB_BLK_RAW) { const u8* p = src + B.src_pos; for (u32 i = lane; i < B.regen; i += 32) bout[i] = p[i]; __syncwarp(); ZB_XMARK(0); continue; }
+        if (B.kind == ZB_BLK_RLE) { for (u32 i = lane; i < B.regen; i += 32) bout[i] = (u8)B.lit_byte; __syncwarp(); ZB_XMARK(0); continue; }
         if (B.kind != ZB_BLK_COMPRESSED) return;
         bool const lit_rle = B.lit_kind == ZB_LIT_RLE; u8 const lit_byte = (u8)B.lit_byte;
         if (B.lit_kind == ZB_LIT_SCRATCH) {               // 16-byte aligned slice of the literal scratch
@@ -952,6 +966,7 @@ zb_execute_tile(const u8* __restrict__ src, const ZbFramePlace* __restrict__ pla
             const u8* g = src + B.src_pos; for (u32 i = lane; i < B.n_lit; i += 32) sl[i] = g[i];
         }
         __syncwarp();
+        ZB_XMARK(0);
         const ZbSeq* const sq = seqs + B.seq_pos;
         u32 const nseq = B.n_seq;
         for (u32 g = 0; g < nseq; g += 32) {
@@ -967,16 +982,24 @@ zb_execute_tile(const u8* __restrict__ src, const ZbFramePlace* __restrict__ pla
                 else zb_copy_fwd8(o, sl + r.x, ll);
             }
             __syncwarp();
+            ZB_XMARK(1);
             bool pending = valid;
             int const abs_m = (int)B.out_pos + (int)mstart;             // frame-relative match start
             int const srcp = abs_m - (int)off;                          // negative: reaches into the dictionary
-            int const need = min(srcp + (int)ml, (int)B.out_pos + (int)ostart);
+            int const need = min(srcp + (int)ml, abs_m);                // bytes [srcp, need) come from other sequences
+            // the group's sequences whose matches start below `need`: lanes [0, t) (match starts ascend with the lane)
+            int const key = valid ? abs_m : 0x7FFFFFFF, mend = abs_m + (int)ml;
+            u32 t = 0;
+            for (u32 b = 16; b; b >>= 1) if (__shfl_sync(0xFFFFFFFFu, key, t + b - 1) < need) t += b;
+            u32 const below = t ? 0xFFFFFFFFu >> (32 - t) : 0u;
             for (;;) {
                 u32 const pm = __ballot_sync(0xFFFFFFFFu, pending);
                 if (!pm) break;
-                int const fu = __ffs(pm) - 1;
-                int const F = __shfl_sync(0xFFFFFFFFu, abs_m, fu);
-                bool const ready = pending && need <= F;
+                // a lane may run when no unfinished match overlaps its source: the last unfinished one starting below
+                // `need` (it ends last: matches are disjoint and in order) ends at or before srcp
+                u32 const cand = pm & below;
+                int const e = __shfl_sync(0xFFFFFFFFu, mend, cand ? 31 - __clz((int)cand) : (int)lane);
+                bool const ready = pending && (!cand || e <= srcp);
                 u32 big = __ballot_sync(0xFFFFFFFFu, ready && ml >= 32);
                 while (big) {
                     int const l = __ffs(big) - 1; big &= big - 1;
@@ -1009,6 +1032,7 @@ zb_execute_tile(const u8* __restrict__ src, const ZbFramePlace* __restrict__ pla
                 }
                 __syncwarp();
             }
+            ZB_XMARK(2);
         }
         {
             ZbSeq const e = sq[nseq];
@@ -1017,6 +1041,7 @@ zb_execute_tile(const u8* __restrict__ src, const ZbFramePlace* __restrict__ pla
             else for (u32 k = lane; k < tail; k += 32) bout[e.y + k] = sl[e.x + k];
         }
         __syncwarp();
+        ZB_XMARK(1);
     }
     // finished frame -> HBM, 128-bit stores (so and dst share the same 16-byte phase)
     {
@@ -1029,6 +1054,8 @@ zb_execute_tile(const u8* __restrict__ src, const ZbFramePlace* __restrict__ pla
         u32 const done = head + (nv << 4);
         if (done + lane < total) out[done + lane] = so[done + lane];
     }
+    ZB_XMARK(3);
+    ZB_XFLUSH();
 }
 
 
@@ -1773,6 +1800,16 @@ void zb_entropy_phase_read(unsigned long long* out8, int reset)
     if (reset) { unsigned long long z[8] = {0}; cudaMemcpyToSymbol(g_zb_ent_phase, z, sizeof z); }
 #else
     for (int i = 0; i < 8; i++) out8[i] = 0; (void)reset;
+#endif
+}
+
+void zb_execute_phase_read(unsigned long long* out4, int reset)
+{
+#ifdef ZB_PHASE_TIMERS
+    cudaMemcpyFromSymbol(out4, g_zb_exe_phase, sizeof(unsigned long long) * 4);
+    if (reset) { unsigned long long z[4] = {0}; cudaMemcpyToSymbol(g_zb_exe_phase, z, sizeof z); }
+#else
+    for (int i = 0; i < 4; i++) out4[i] = 0; (void)reset;
 #endif
 }
 

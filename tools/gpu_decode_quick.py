@@ -29,8 +29,13 @@ tot = sum(v[0] / v[1] for v in p.values())
 print({k: round(v[0] / v[1], 3) for k, v in p.items()}, "total ms %.3f -> %.1f GB/s" % (tot, len(blob) / tot / 1e6))
 if os.environ.get("PHASES"):
     L.zb_entropy_phase_read.argtypes = [C.c_void_p, C.c_int]
+    L.zb_execute_phase_read.argtypes = [C.c_void_p, C.c_int]
     buf = (C.c_uint64 * 8)(); L.zb_entropy_phase_read(buf, 1)
-    L.zb200_result_free(step()); L.zb_entropy_phase_read(buf, 1)
+    xbuf = (C.c_uint64 * 4)(); L.zb_execute_phase_read(xbuf, 1)
+    L.zb200_result_free(step()); L.zb_entropy_phase_read(buf, 1); L.zb_execute_phase_read(xbuf, 1)
     names = ['other/loop', 'A block header', 'B literals hdr+weights', 'huffman table+streams', 'C seq header+ncount', 'D tables+sequences']
     tot = float(sum(buf[i] for i in range(6))) or 1.0
     print('entropy phases (share of summed warp cycles):', {nm: "%.1f%%" % (100.0 * buf[i] / tot) for i, nm in enumerate(names)}, "sum Mcycles %.0f" % (tot / 1e6))
+    xnames = ['frame start + literal staging', 'literal copies', 'frontier passes', 'write-out']
+    print('zb_execute_tile phases (summed warp cycles):', {nm: "%.1f Mcycles" % (xbuf[i] / 1e6) for i, nm in enumerate(xnames)},
+          "sum Mcycles %.0f" % (sum(xbuf[i] for i in range(4)) / 1e6))

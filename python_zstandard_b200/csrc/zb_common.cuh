@@ -96,6 +96,10 @@ typedef u32 ZbFseCell;
 #define ZB_CELL_NB(c)   (((c) >> 10) & 15u)
 #define ZB_CELL_ADD(c)  (((c) >> 14) & 31u)
 #define ZB_CELL_SYM(c)  ((c) >> 19)
+// The entropy kernels' sequence loop reads 16-bit cells instead, so that a lane's three tables take half the shared
+// memory: symbol | x << 6, with x the state's occurrence count (< 2^(log + 1)).  nbBits = log - hibit(x), next state
+// base = (x << nbBits) - 2^log, the extra-bit count comes from the symbol.  From a 32-bit cell: x = (next + 2^log) >> nb.
+#define ZB_CELL16(sym, x) ((u16)((sym) | ((x) << 6)))
 
 // digested dictionary, device resident (restates what ZSTD_loadDEntropy keeps, zstd/zstd.c:44673-44757)
 struct ZbDictDev {
@@ -157,10 +161,12 @@ template <int N> __device__ __forceinline__ void zb_cp_wait()         // all but
 // [16k, 16k + 16) above the 16-byte aligned base -- in slot k mod D), which asynchronous copies keep
 // filled ahead of the decode: a refill that moves into chunk k requests chunk k + 1 - D, whose first
 // word is needed 4D - 7 refills later at the earliest (4D - 4 in steady state, less right after
-// init).  Every refill commits one copy group and, before it reads the ring, waits for all but the
+// init): a refill moves at most one word into the window, however many bits were read since the
+// last one.  Every refill commits one copy group and, before it reads the ring, waits for all but the
 // 4D - 8 most recent groups of the thread; other readers' refills in between only add groups.  So a
-// copy has 4(D - 1) refills of decode to land in, which a 4-byte load issued one word ahead (one or
-// two sequence steps) could not get: lanes of a warp refill at different moments and the warp's
+// copy has 4(D - 1) refills of decode to land in -- in the sequence decoder, which refills once per
+// sequence in the common case, that many sequences at least -- where a 4-byte load issued one word ahead
+// could not hide its latency: lanes of a warp refill at different moments and the warp's
 // load scoreboard made nearly every refill wait for the latest lane's load.  The cp.async groups
 // are ordered, so the wait is for copies that are old.
 //

@@ -416,23 +416,26 @@ __device__ __forceinline__ u32 zb_code_add_bits(u32 sym, int kind)
     return kind == K_LL ? c_LL_bits[sym] : (kind == K_ML ? c_ML_bits[sym] : sym);
 }
 
-// tANS decode table of 32-bit cells (restates ZSTD_buildFSETable_body, zstd/zstd.c:46118-46233), serial.
+// tANS decode table (restates ZSTD_buildFSETable_body, zstd/zstd.c:46118-46233), serial.
 // `norm` (max_sym + 1 shorts) is consumed: it becomes the per-symbol next-state counters in place.
-__device__ static void zb_build_fse(ZbFseCell* t, short* norm, u32 max_sym, u32 log, int kind)
+// Cells: 32-bit ZbFseCell, or the entropy kernels' 16-bit ZB_CELL16.
+template <typename Cell = ZbFseCell>
+__device__ static void zb_build_fse(Cell* t, short* norm, u32 max_sym, u32 log, int kind)
 {
     u32 const size = 1u << log, mask = size - 1, step = (size >> 1) + (size >> 3) + 3;
     u32 high = size - 1;
-    for (u32 s = 0; s <= max_sym; s++) if (norm[s] == -1) { t[high--] = s; norm[s] = 0x4001; }
+    for (u32 s = 0; s <= max_sym; s++) if (norm[s] == -1) { t[high--] = (Cell)s; norm[s] = 0x4001; }
     u32 pos = 0;
     for (u32 s = 0; s <= max_sym; s++) {
         int const c = norm[s];
         if (c & 0x4000) { norm[s] = 1; continue; }
-        for (int i = 0; i < c; i++) { t[pos] = s; do pos = (pos + step) & mask; while (pos > high); }
+        for (int i = 0; i < c; i++) { t[pos] = (Cell)s; do pos = (pos + step) & mask; while (pos > high); }
     }
     for (u32 u = 0; u < size; u++) {
         u32 const s = t[u], x = (u32)(u16)norm[s]; norm[s] = (short)(x + 1);
         u32 const nb = log - (u32)zb_hibit(x);
-        t[u] = ZB_CELL((x << nb) - size, nb, zb_code_add_bits(s, kind), s);
+        if constexpr (sizeof(Cell) == 4) t[u] = ZB_CELL((x << nb) - size, nb, zb_code_add_bits(s, kind), s);
+        else t[u] = ZB_CELL16(s, x);
     }
 }
 
@@ -449,7 +452,7 @@ __global__ void zb_build_default_tables()
     }
 }
 
-struct ZbTab { const ZbFseCell* t; u32 log; };
+struct ZbTab { u32 off; u32 log; };         // off: byte offset of the cells in the entropy kernels' shared memory
 
 #include "zb_entropy.cuh"
 

@@ -17,14 +17,22 @@
 #pragma once
 
 // Warps per CTA (one CTA per SM) is a template parameter: each warp owns a shared-memory pool of
-// (227 KB - LUT) / warps.  Level-3 frames of a few KiB carry three 64-cell FSE tables (768 B per lane) and a ~600 B
-// Huffman table: 8 warps (28.9 KB pools) serve them best; frames of 16 KiB and more have larger tables and run faster
-// with 7 warps and 33 KB pools (measured 7.2 vs 8.8 ms on 65536 x 16 KiB), since a lane whose tables do not fit waits
+// (227 KB - head) / warps.  Level-3 frames of a few KiB carry three FSE tables of 64-128 cells (~500 B per lane in 16-bit
+// cells, so that all 32 lanes of a warp fit in one pass) and a ~600 B Huffman table: 8 warps (28.9 KB pools) serve them
+// best; frames of 16 KiB and more have larger tables and run faster with 7 warps and 33 KB pools (measured 7.2 vs 8.8 ms on 65536 x 16 KiB), since a lane whose tables do not fit waits
 // for a second pass.
+//
+// In front of the pools sits a CTA-wide head: the LL / ML baseline LUTs, the three predefined FSE tables and, when the
+// dictionary carries entropy tables, the dictionary's three FSE tables (at most 2.5 KB, taken from the pools of that call),
+// all in 16-bit cells (ZB_CELL16).  So every table the sequence loop reads is in shared memory and is addressed by a
+// 32-bit offset: its cell loads are LDS.
 #define ZB_ENT_WS_BYTES   256                     // per-lane workspace (weights / normalized counts)
-#define ZB_ENT_POOL_BYTES(W) ((((227 * 1024 - 512) / (W))) & ~15)
-#define ZB_ENT_LUT_BYTES  512                     // CTA-wide baseline tables (LL_base, ML_base)
-#define ZB_ENT_SMEM(W)    ((W) * ZB_ENT_POOL_BYTES(W) + ZB_ENT_LUT_BYTES)
+#define ZB_ENT_DEF_LL     512                     // after the baselines (LL_base, ML_base): predefined LL, OF, ML cells
+#define ZB_ENT_DEF_OF     (ZB_ENT_DEF_LL + 2 * 64)
+#define ZB_ENT_DEF_ML     (ZB_ENT_DEF_OF + 2 * 32)
+#define ZB_ENT_HEAD_BYTES (ZB_ENT_DEF_ML + 2 * 64)  // the dictionary's tables follow, when there are any
+#define ZB_ENT_POOL_BYTES(W) ((((227 * 1024 - ZB_ENT_HEAD_BYTES) / (W))) & ~15)
+#define ZB_ENT_SMEM(W)    ((W) * ZB_ENT_POOL_BYTES(W) + ZB_ENT_HEAD_BYTES)
 
 // where a table comes from; enough to rebuild it for a later block
 enum : u32 { ZB_SRC_NONE = 0, ZB_SRC_PREDEF = 1, ZB_SRC_RLE = 2, ZB_SRC_NCOUNT = 3, ZB_SRC_DICT = 4 };
@@ -248,9 +256,134 @@ __device__ static int zb_seq_desc(ZbTabSrc& d, u32 mode, u32 max_sym_kind, u32 m
         u32 const u = zb_read_ncount(norm, max_sym, log, d.p, d.n);
         if (u == 0 || log > max_log) return -1;
         if (mode == 2) { used = (int)u; d.n = u; }
-        need = 4u << log;
-    } else if (d.kind == ZB_SRC_RLE) need = 4;
+        need = 2u << log;                                   // 16-bit cells
+    } else if (d.kind == ZB_SRC_RLE) need = 2;
     return used;
+}
+
+// i = 0 .. n-1 spread over the CTA's threads
+template <class F> __device__ __forceinline__ void zb_cta_for(u32 n, F f)
+{
+#ifdef __CUDA_ARCH__
+    for (u32 i = threadIdx.x; i < n; i += blockDim.x) f(i);
+#else
+    if (threadIdx.x == 0) for (u32 i = 0; i < n; i++) f(i);       // a CPU build may run thread 0 alone
+#endif
+}
+
+// 32-bit cells of a table of 2^log -> ZB_CELL16 cells
+__device__ __forceinline__ void zb_cta_cells16(u8* dst, const ZbFseCell* src, u32 log)
+{
+    zb_cta_for(1u << log, [&](u32 i) { u32 const c = src[i]; ((u16*)dst)[i] = ZB_CELL16(ZB_CELL_SYM(c), (ZB_CELL_NEXT(c) + (1u << log)) >> ZB_CELL_NB(c)); });
+}
+
+// Fill the CTA-wide head of the entropy kernels' shared memory (see ZB_ENT_HEAD_BYTES); returns the bytes of each warp's pool.
+// The baseline LUTs carry the symbol's extra-bit count in bits 24-31.
+template <int W>
+__device__ __forceinline__ u32 zb_ent_head(u8* smem, ZbDictDev const& dict)
+{
+    u32* const lutLL = (u32*)smem; u32* const lutML = lutLL + 36;      // indexed by symbol code
+    zb_cta_for(36, [&](u32 i) { lutLL[i] = c_LL_base[i] | ((u32)c_LL_bits[i] << 24); });
+    zb_cta_for(53, [&](u32 i) { lutML[i] = c_ML_base[i] | ((u32)c_ML_bits[i] << 24); });
+    zb_cta_cells16(smem + ZB_ENT_DEF_LL, g_defLL, 6);
+    zb_cta_cells16(smem + ZB_ENT_DEF_OF, g_defOF, 5);
+    zb_cta_cells16(smem + ZB_ENT_DEF_ML, g_defML, 6);
+    u32 head = ZB_ENT_HEAD_BYTES;
+    if (dict.has_entropy) {                                            // logs <= 9, 8, 9 (zb_digest_dict)
+        zb_cta_cells16(smem + head, dict.ll, dict.ll_log); head += 2u << dict.ll_log;
+        zb_cta_cells16(smem + head, dict.of, dict.of_log); head += 2u << dict.of_log;
+        zb_cta_cells16(smem + head, dict.ml, dict.ml_log); head += 2u << dict.ml_log;
+    }
+    __syncthreads();
+    return ((ZB_ENT_SMEM(W) - head) / W) & ~15u;
+}
+
+// -- D of one block in one lane: place the three FSE tables (built at q in the lane's pool claim, or the predefined or the
+// dictionary's ones in the head), then run the 3-state sequence stream (restates ZSTD_decodeSequence, zstd/zstd.c:46862-46986)
+// into sq[0, nseq).  Returns the error code; lit_used / produced / rep0..2 carry the block's totals and repcode history out.
+// SYMREP: the history may be symbolic (zb_entropy_blocks: 0x80000000 | k << 29 | d stands for "entry repcode k, minus d").
+//
+// The bit window holds 32..64 bits after a refill, while a sequence takes ~16 on 4 KiB level-3 frames.  So the sequence refills
+// once, after its cell loads, and reads its offset, ML + LL and state bits without refilling in between when they all fit in
+// the window; otherwise it refills before each of the last two reads as well.  Either way every read sees the same bits as
+// with a refill before each read, and left() and its checks are unchanged.
+template <bool SYMREP>
+__device__ __forceinline__ u32 zb_seq_block(const u8* smem, u8* q, u8* ws, ZbDictDev const& dict,
+                                            ZbTabSrc const& dLL, ZbTabSrc const& dOF, ZbTabSrc const& dML,
+                                            u32 msLL, u32 msOF, u32 msML, u32 logLL, u32 logOF, u32 logML,
+                                            const u8* ip, const u8* bend, u32 nseq, ZbSeq* sq, u32 n_lit, u64 room, u64 hist,
+                                            u32& rep0, u32& rep1, u32& rep2, u32& lit_used, u32& produced)
+{
+    const u32* const lutLL = (const u32*)smem; const u32* const lutML = lutLL + 36;
+    short* const normLL = (short*)ws; short* const normOF = normLL + 36; short* const normML = normOF + 32;
+    u32 const dct_ll = ZB_ENT_HEAD_BYTES, dct_of = dct_ll + (2u << dict.ll_log), dct_ml = dct_of + (2u << dict.of_log);
+    ZbTab tLL, tOF, tML;
+    auto setup = [&](const ZbTabSrc& d, short* norm, u32 ms, u32 lg, int kind, u32 dct, u32 dlog, u32 def, u32 deflog, ZbTab& t) {
+        if (d.kind == ZB_SRC_NCOUNT) { zb_build_fse((u16*)q, norm, ms, lg, kind); t.off = (u32)(q - smem); t.log = lg; q += 2u << lg; }
+        else if (d.kind == ZB_SRC_RLE) { *(u16*)q = ZB_CELL16(d.sym, 1u); t.off = (u32)(q - smem); t.log = 0; q += 2; }
+        else if (d.kind == ZB_SRC_DICT) { t.off = dct; t.log = dlog; }
+        else { t.off = def; t.log = deflog; }
+    };
+    setup(dLL, normLL, msLL, logLL, K_LL, dct_ll, dict.ll_log, ZB_ENT_DEF_LL, 6, tLL);
+    setup(dOF, normOF, msOF, logOF, K_OF, dct_of, dict.of_log, ZB_ENT_DEF_OF, 5, tOF);
+    setup(dML, normML, msML, logML, K_ML, dct_ml, dict.ml_log, ZB_ENT_DEF_ML, 6, tML);
+
+    ZbBitR<8> b;                        // ring: the lane workspace (the normalized counts are consumed)
+    if (!b.init(ip, (u32)(bend - ip), ws)) return ZB_E_CORRUPTION;
+    u32 sLL = b.read(tLL.log); u32 sOF = b.read(tOF.log); b.refill(); u32 sML = b.read(tML.log);
+    const u8* const TL = smem + tLL.off; const u8* const TO = smem + tOF.off; const u8* const TM = smem + tML.off;
+    u32 const kL = 31 - tLL.log, kO = 31 - tOF.log, kM = 31 - tML.log;                 // nbBits = clz(x) - k
+    u32 err = ZB_OK;
+    for (u32 i = 0; i < nseq; i++) {
+        u32 const cl = *(const u16*)(TL + 2 * sLL), co = *(const u16*)(TO + 2 * sOF), cm = *(const u16*)(TM + 2 * sML);
+        b.refill();
+        u32 const llc = cl & 63, ofc = co & 63, xl = cl >> 6, xo = co >> 6, xm = cm >> 6;
+        u32 const nl = __clz(xl) - kL, nm = __clz(xm) - kM, no = __clz(xo) - kO;
+        u32 const eL = lutLL[llc], eM = lutML[cm & 63];            // baseline | extra bits << 24: off the state chain
+        u32 const llb = eL >> 24, ab = (eM >> 24) + llb;                                 // ML then LL additional bits (<= 32)
+        u32 const sb = i + 1 < nseq ? nl + nm + no : 0;                                  // the three state updates (<= 26)
+        bool const slow = (int)(ofc + ab + sb) > b.avail;                                 // ofc: the offset's extra bits
+        u32 const ob = b.read(ofc);
+        u32 ll = eL & 0xFFFFFFu, ml = eM & 0xFFFFFFu, off;
+        // (a branch-free select chain over {rep0, rep1, rep2, rep0 - 1, new} was measured 3-5 % slower than this branch)
+        if (ofc > 1) {
+            off = (1u << ofc) - 3 + ob;
+            rep2 = rep1; rep1 = rep0; rep0 = off;
+        } else {
+            u32 const ll0 = (llc == 0);
+            if (ofc == 0) {
+                if (ll0) { off = rep1; rep1 = rep0; rep0 = off; } else off = rep0;
+            } else {
+                u32 const idx = 1 + ll0 + ob;
+                u32 const r0m = SYMREP && (rep0 & 0x80000000u) ? rep0 + 1 : rep0 - 1;   // symbolic: one more off
+                u32 tmp = idx == 1 ? rep1 : (idx == 2 ? rep2 : r0m);
+                if (tmp == 0) tmp = 0xFFFFFFFFu;
+                if (idx != 1) rep2 = rep1;
+                rep1 = rep0; rep0 = off = tmp;
+            }
+        }
+        if (slow) b.refill();
+        {
+            u32 const both = b.read(ab);
+            ml += both >> llb; ll += both & ((1u << llb) - 1);
+        }
+        if (slow) b.refill();
+        {   // LL, ML, OF in one read
+            u32 const v = b.read(sb);
+            sLL = (xl << nl) - (1u << tLL.log) + (v >> (nm + no));
+            sML = (xm << nm) - (1u << tML.log) + ((v >> no) & ((1u << nm) - 1));
+            sOF = (xo << no) - (1u << tOF.log) + (v & ((1u << no) - 1));
+        }
+        sq[i] = make_uint4(lit_used, produced, ml, off);
+        // the checks of ZSTD_execSequence / ZSTD_execSequenceEnd (zstd/zstd.c:46540-46728)
+        if ((u64)produced + ll + ml > room) { err = ZB_E_DSTSIZE_TOO_SMALL; break; }
+        if (ll > n_lit - lit_used) { err = ZB_E_CORRUPTION; break; }
+        lit_used += ll; produced += ll;
+        if ((u64)off > hist + produced) { err = ZB_E_CORRUPTION; break; }
+        produced += ml;
+    }
+    if (!err && b.left() != 0) err = ZB_E_CORRUPTION;
+    return err;
 }
 
 // per-phase cycle counters (lane 0 of every warp) exist only in tuning builds (-DZB_PHASE_TIMERS)
@@ -273,14 +406,11 @@ zb_entropy_decode(const u8* __restrict__ src, const ZbSegment* __restrict__ segs
 {
     extern __shared__ __align__(16) u8 zb_smem[];
     u32 const lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    u32* const lutLL = (u32*)zb_smem; u32* const lutML = lutLL + 36;      // baselines, indexed by symbol code
-    if (threadIdx.x < 36) lutLL[threadIdx.x] = c_LL_base[threadIdx.x];
-    if (threadIdx.x < 53) lutML[threadIdx.x] = c_ML_base[threadIdx.x];
-    __syncthreads();
-    u8* const pool = zb_smem + ZB_ENT_LUT_BYTES + warp * ZB_ENT_POOL_BYTES(ZB_ENT_WARPS);
+    u32 const pool_bytes = zb_ent_head<ZB_ENT_WARPS>(zb_smem, dict);
+    u8* const pool = zb_smem + ZB_ENT_SMEM(ZB_ENT_WARPS) - (ZB_ENT_WARPS - warp) * pool_bytes;      // pools: behind the head
     u8* const ws = pool + lane * ZB_ENT_WS_BYTES;                       // lane workspace
     u8* const tabs = pool + 32 * ZB_ENT_WS_BYTES;                       // claimable table space
-    u32 const TAB_BYTES = ZB_ENT_POOL_BYTES(ZB_ENT_WARPS) - 32 * ZB_ENT_WS_BYTES;
+    u32 const TAB_BYTES = pool_bytes - 32 * ZB_ENT_WS_BYTES;
 
     for (;;) {
         u32 base = 0;
@@ -437,71 +567,9 @@ zb_entropy_decode(const u8* __restrict__ src, const ZbSegment* __restrict__ segs
                     u32 const need = pending ? ((needS + 15) & ~15u) : 0;
                     u32 const incl = zb_warp_incl_scan(need, lane);
                     if (pending && incl <= TAB_BYTES) {
-                        u8* q = tabs + incl - need;
-                        ZbTab tLL, tOF, tML;
-                        auto setup = [&](const ZbTabSrc& d, short* norm, u32 ms, u32 lg, int kind, const ZbFseCell* dct, u32 dlog,
-                                         const ZbFseCell* def, u32 deflog, ZbTab& t) {
-                            if (d.kind == ZB_SRC_NCOUNT) { zb_build_fse((ZbFseCell*)q, norm, ms, lg, kind); t.t = (ZbFseCell*)q; t.log = lg; q += 4u << lg; }
-                            else if (d.kind == ZB_SRC_RLE) { *(ZbFseCell*)q = ZB_CELL(0, 0, zb_code_add_bits(d.sym, kind), d.sym); t.t = (ZbFseCell*)q; t.log = 0; q += 4; }
-                            else if (d.kind == ZB_SRC_DICT) { t.t = dct; t.log = dlog; }
-                            else { t.t = def; t.log = deflog; }
-                        };
-                        setup(dLL, normLL, msLL, logLL, K_LL, dict.ll, dict.ll_log, g_defLL, 6, tLL);
-                        setup(dOF, normOF, msOF, logOF, K_OF, dict.of, dict.of_log, g_defOF, 5, tOF);
-                        setup(dML, normML, msML, logML, K_ML, dict.ml, dict.ml_log, g_defML, 6, tML);
-
-                        // the 3-state FSE sequence stream (restates ZSTD_decodeSequence, zstd/zstd.c:46862-46986)
-                        ZbBitR<8> b;                        // ring: the lane workspace (the normalized counts are consumed)
-                        if (!b.init(ip, (u32)(bend - ip), ws)) err = ZB_E_CORRUPTION;
-                        else {
-                            u32 sLL = b.read(tLL.log); u32 sOF = b.read(tOF.log); b.refill(); u32 sML = b.read(tML.log); b.refill();
-                            const ZbFseCell* const TL = tLL.t; const ZbFseCell* const TO = tOF.t; const ZbFseCell* const TM = tML.t;
-                            u64 const room = cap - out_pos;
-                            ZbSeq* const sq = seqs + seq_i;
-                            for (u32 i = 0; i < nseq; i++) {
-                                u32 const cl = TL[sLL], co = TO[sOF], cm = TM[sML];
-                                u32 const ofc = ZB_CELL_SYM(co), llc = ZB_CELL_SYM(cl);
-                                u32 ll = lutLL[llc], ml = lutML[ZB_CELL_SYM(cm)], off;      // baselines: off the state chain
-                                // (a branch-free select chain over {rep0, rep1, rep2, rep0 - 1, new} was measured 3-5 % slower than this branch)
-                                if (ofc > 1) {
-                                    off = (1u << ofc) - 3 + b.read(ofc);
-                                    rep2 = rep1; rep1 = rep0; rep0 = off;
-                                } else {
-                                    u32 const ll0 = (llc == 0);
-                                    if (ofc == 0) {
-                                        if (ll0) { off = rep1; rep1 = rep0; rep0 = off; } else off = rep0;
-                                    } else {
-                                        u32 const idx = 1 + ll0 + b.read(1);
-                                        u32 tmp = idx == 1 ? rep1 : (idx == 2 ? rep2 : rep0 - 1);
-                                        if (tmp == 0) tmp = 0xFFFFFFFFu;
-                                        if (idx != 1) rep2 = rep1;
-                                        rep1 = rep0; rep0 = off = tmp;
-                                    }
-                                }
-                                b.refill();
-                                {   // ML then LL additional bits in one read (<= 32 bits)
-                                    u32 const llb = ZB_CELL_ADD(cl), both = b.read(ZB_CELL_ADD(cm) + llb);
-                                    ml += both >> llb; ll += both & ((1u << llb) - 1);
-                                }
-                                b.refill();
-                                if (i + 1 < nseq) {   // the three state updates (LL, ML, OF) in one read (<= 26 bits)
-                                    u32 const nl = ZB_CELL_NB(cl), nm = ZB_CELL_NB(cm), no = ZB_CELL_NB(co);
-                                    u32 const v = b.read(nl + nm + no);
-                                    sLL = ZB_CELL_NEXT(cl) + (v >> (nm + no));
-                                    sML = ZB_CELL_NEXT(cm) + ((v >> no) & ((1u << nm) - 1));
-                                    sOF = ZB_CELL_NEXT(co) + (v & ((1u << no) - 1));
-                                    b.refill();
-                                }
-                                sq[i] = make_uint4(lit_used, produced, ml, off);
-                                // the checks of ZSTD_execSequence / ZSTD_execSequenceEnd (zstd/zstd.c:46540-46728)
-                                if ((u64)produced + ll + ml > room) { err = ZB_E_DSTSIZE_TOO_SMALL; break; }
-                                if (ll > L.regen - lit_used) { err = ZB_E_CORRUPTION; break; }
-                                lit_used += ll; produced += ll;
-                                if ((u64)off > out_pos + produced + hist_extra) { err = ZB_E_CORRUPTION; break; }
-                                produced += ml;
-                            }
-                            if (!err && b.left() != 0) err = ZB_E_CORRUPTION;
-                        }
+                        err = zb_seq_block<false>(zb_smem, tabs + incl - need, ws, dict, dLL, dOF, dML, msLL, msOF, msML, logLL, logOF, logML,
+                                                   ip, bend, nseq, seqs + seq_i, L.regen, cap - out_pos, out_pos + hist_extra,
+                                                   rep0, rep1, rep2, lit_used, produced);
                         if (err) { done = true; comp = false; }
                         pending = false;
                     }
@@ -557,14 +625,11 @@ zb_entropy_blocks(const u8* __restrict__ src, const ZbBlkDesc* __restrict__ bdes
 {
     extern __shared__ __align__(16) u8 zb_smem[];
     u32 const lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    u32* const lutLL = (u32*)zb_smem; u32* const lutML = lutLL + 36;      // baselines, indexed by symbol code
-    if (threadIdx.x < 36) lutLL[threadIdx.x] = c_LL_base[threadIdx.x];
-    if (threadIdx.x < 53) lutML[threadIdx.x] = c_ML_base[threadIdx.x];
-    __syncthreads();
-    u8* const pool = zb_smem + ZB_ENT_LUT_BYTES + warp * ZB_ENT_POOL_BYTES(ZB_ENT_WARPS);
+    u32 const pool_bytes = zb_ent_head<ZB_ENT_WARPS>(zb_smem, dict);
+    u8* const pool = zb_smem + ZB_ENT_SMEM(ZB_ENT_WARPS) - (ZB_ENT_WARPS - warp) * pool_bytes;      // pools: behind the head
     u8* const ws = pool + lane * ZB_ENT_WS_BYTES;                       // lane workspace
     u8* const tabs = pool + 32 * ZB_ENT_WS_BYTES;                       // claimable table space
-    u32 const TAB_BYTES = ZB_ENT_POOL_BYTES(ZB_ENT_WARPS) - 32 * ZB_ENT_WS_BYTES;
+    u32 const TAB_BYTES = pool_bytes - 32 * ZB_ENT_WS_BYTES;
 
     for (;;) {
         u32 base = 0;
@@ -721,71 +786,9 @@ zb_entropy_blocks(const u8* __restrict__ src, const ZbBlkDesc* __restrict__ bdes
                     u32 const need = pending ? ((needS + 15) & ~15u) : 0;
                     u32 const incl = zb_warp_incl_scan(need, lane);
                     if (pending && incl <= TAB_BYTES) {
-                        u8* q = tabs + incl - need;
-                        ZbTab tLL, tOF, tML;
-                        auto setup = [&](const ZbTabSrc& d, short* norm, u32 ms, u32 lg, int kind, const ZbFseCell* dct, u32 dlog,
-                                         const ZbFseCell* def, u32 deflog, ZbTab& t) {
-                            if (d.kind == ZB_SRC_NCOUNT) { zb_build_fse((ZbFseCell*)q, norm, ms, lg, kind); t.t = (ZbFseCell*)q; t.log = lg; q += 4u << lg; }
-                            else if (d.kind == ZB_SRC_RLE) { *(ZbFseCell*)q = ZB_CELL(0, 0, zb_code_add_bits(d.sym, kind), d.sym); t.t = (ZbFseCell*)q; t.log = 0; q += 4; }
-                            else if (d.kind == ZB_SRC_DICT) { t.t = dct; t.log = dlog; }
-                            else { t.t = def; t.log = deflog; }
-                        };
-                        setup(dLL, normLL, msLL, logLL, K_LL, dict.ll, dict.ll_log, g_defLL, 6, tLL);
-                        setup(dOF, normOF, msOF, logOF, K_OF, dict.of, dict.of_log, g_defOF, 5, tOF);
-                        setup(dML, normML, msML, logML, K_ML, dict.ml, dict.ml_log, g_defML, 6, tML);
-
-                        // the 3-state FSE sequence stream (restates ZSTD_decodeSequence, zstd/zstd.c:46862-46986)
-                        ZbBitR<8> b;                        // ring: the lane workspace (the normalized counts are consumed)
-                        if (!b.init(ip, (u32)(bend - ip), ws)) err = ZB_E_CORRUPTION;
-                        else {
-                            u32 sLL = b.read(tLL.log); u32 sOF = b.read(tOF.log); b.refill(); u32 sML = b.read(tML.log); b.refill();
-                            const ZbFseCell* const TL = tLL.t; const ZbFseCell* const TO = tOF.t; const ZbFseCell* const TM = tML.t;
-                            u64 const room = cap - out_pos;
-                            ZbSeq* const sq = seqs + seq_i;
-                            for (u32 i = 0; i < nseq; i++) {
-                                u32 const cl = TL[sLL], co = TO[sOF], cm = TM[sML];
-                                u32 const ofc = ZB_CELL_SYM(co), llc = ZB_CELL_SYM(cl);
-                                u32 ll = lutLL[llc], ml = lutML[ZB_CELL_SYM(cm)], off;      // baselines: off the state chain
-                                // (a branch-free select chain over {rep0, rep1, rep2, rep0 - 1, new} was measured 3-5 % slower than this branch)
-                                if (ofc > 1) {
-                                    off = (1u << ofc) - 3 + b.read(ofc);
-                                    rep2 = rep1; rep1 = rep0; rep0 = off;
-                                } else {
-                                    u32 const ll0 = (llc == 0);
-                                    if (ofc == 0) {
-                                        if (ll0) { off = rep1; rep1 = rep0; rep0 = off; } else off = rep0;
-                                    } else {
-                                        u32 const idx = 1 + ll0 + b.read(1);
-                                        u32 tmp = idx == 1 ? rep1 : (idx == 2 ? rep2 : ((rep0 & 0x80000000u) ? rep0 + 1 : rep0 - 1));     // symbolic: one more off
-                                        if (tmp == 0) tmp = 0xFFFFFFFFu;
-                                        if (idx != 1) rep2 = rep1;
-                                        rep1 = rep0; rep0 = off = tmp;
-                                    }
-                                }
-                                b.refill();
-                                {   // ML then LL additional bits in one read (<= 32 bits)
-                                    u32 const llb = ZB_CELL_ADD(cl), both = b.read(ZB_CELL_ADD(cm) + llb);
-                                    ml += both >> llb; ll += both & ((1u << llb) - 1);
-                                }
-                                b.refill();
-                                if (i + 1 < nseq) {   // the three state updates (LL, ML, OF) in one read (<= 26 bits)
-                                    u32 const nl = ZB_CELL_NB(cl), nm = ZB_CELL_NB(cm), no = ZB_CELL_NB(co);
-                                    u32 const v = b.read(nl + nm + no);
-                                    sLL = ZB_CELL_NEXT(cl) + (v >> (nm + no));
-                                    sML = ZB_CELL_NEXT(cm) + ((v >> no) & ((1u << nm) - 1));
-                                    sOF = ZB_CELL_NEXT(co) + (v & ((1u << no) - 1));
-                                    b.refill();
-                                }
-                                sq[i] = make_uint4(lit_used, produced, ml, off);
-                                // the checks of ZSTD_execSequence / ZSTD_execSequenceEnd (zstd/zstd.c:46540-46728)
-                                if ((u64)produced + ll + ml > room) { err = ZB_E_DSTSIZE_TOO_SMALL; break; }
-                                if (ll > L.regen - lit_used) { err = ZB_E_CORRUPTION; break; }
-                                lit_used += ll; produced += ll;
-                                if ((u64)off > out_pos + produced + hist_extra) { err = ZB_E_CORRUPTION; break; }
-                                produced += ml;
-                            }
-                            if (!err && b.left() != 0) err = ZB_E_CORRUPTION;
-                        }
+                        err = zb_seq_block<true>(zb_smem, tabs + incl - need, ws, dict, dLL, dOF, dML, msLL, msOF, msML, logLL, logOF, logML,
+                                                   ip, bend, nseq, seqs + seq_i, L.regen, cap - out_pos, out_pos + hist_extra,
+                                                   rep0, rep1, rep2, lit_used, produced);
                         if (err) { done = true; comp = false; }
                         pending = false;
                     }

@@ -409,7 +409,7 @@ static int run_decompress(zb200_ctx* ctx, const u8* d_src, const ZbSegment* d_se
     { KSpan s(ctx, ZB200_K_PLACE);
       zb_launch_place(ctx->info.as<ZbFrameInfo>(), d_dst_sizes, nf, ctx->place.as<ZbFramePlace>(), d_totals,
                       ctx->status.as<u32>(), ctx->partial.as<u64>(), ctx->stream); }
-    u64 totals[5];
+    u64 totals[6];          // output, blocks, sequences, literals, any checksum, any window >= ZB_FAR_WINDOW
     CK(cudaMemcpyAsync(totals, d_totals, sizeof totals, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
 
@@ -442,8 +442,11 @@ static int run_decompress(zb200_ctx* ctx, const u8* d_src, const ZbSegment* d_se
     // Measured (tools/gpu_c3_decode.py, tools/gpu_c5_frame.py): frames of one 128 KiB chunk -- the reference's single block or
     // our ten sub-blocks -- are faster a lane per frame at any batch size (2048 of ours: 18.4 vs 6.6 GB/s); from a few full
     // blocks per frame on the lane's serial chain (4-5 ms per 128 KiB) is what the block path removes.
+    // The block path tags symbolic repcodes with bit 31 and rejects larger offsets, so it never takes a batch in which an
+    // offset can reach 2^31: a frame with a window of ZB_FAR_WINDOW or more, or a dictionary of ZB_FAR_DICT bytes or more.
     int const force_blocks = getenv("ZB200_BLOCK_PATH") ? atoi(getenv("ZB200_BLOCK_PATH")) : -1;      // (read per call: tests switch it)
-    bool const block_path = force_blocks >= 0 ? force_blocks != 0 : (totals[1] > n && n < 3000 && totals[0] >= (u64)n * (512u << 10));
+    bool const far = totals[5] != 0 || dd.content_size >= ZB_FAR_DICT;
+    bool const block_path = !far && (force_blocks >= 0 ? force_blocks != 0 : (totals[1] > n && n < 3000 && totals[0] >= (u64)n * (512u << 10)));
     bool chase_path = false;
     ctx->last_chase_rounds = 0;
     if (block_path) {

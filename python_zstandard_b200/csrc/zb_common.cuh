@@ -52,8 +52,14 @@ struct ZbFrameInfo {
     u32 n_blocks;
     u32 status;
     u32 dict_id;
-    u32 flags;            // bit0: checksum present
+    u32 flags;            // bit0: checksum present; bit1: window >= ZB_FAR_WINDOW
 };
+
+// The block-parallel entropy path tags symbolic repcodes with bit 31, so it needs every offset below 2^31.  A frame's offsets
+// stay below its window plus the dictionary content; frames with a window of at least ZB_FAR_WINDOW, and dictionaries of
+// ZB_FAR_DICT bytes or more, keep the batch on the lane-per-frame path.
+#define ZB_FAR_WINDOW  ((1ull << 31) - (1ull << 27))
+#define ZB_FAR_DICT    (1ull << 27)
 
 // per-frame placement, produced by the offsets scan
 struct ZbFramePlace {

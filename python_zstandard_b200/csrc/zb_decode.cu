@@ -142,6 +142,9 @@ __device__ static u32 zb_scan_block_counts(const u8* bs, u32 bsize, u64& n_lit, 
     return ZB_OK;
 }
 
+// ZbFrameInfo.flags of a parsed header (both frame scans write it)
+__device__ __forceinline__ u32 zb_info_flags(ZbHdr const& h) { return h.checksum | (h.window >= ZB_FAR_WINDOW ? 2u : 0u); }
+
 // K1 for one big frame per warp: lane 0 walks the block-header chain 32 blocks ahead (one dependent load per block), then
 // every lane parses the sections of its block.
 __global__ void __launch_bounds__(128)
@@ -156,7 +159,7 @@ zb_scan_frames_big(const u8* __restrict__ src, const ZbSegment* __restrict__ seg
         const u8* s = src + segs[f].offset; u64 n = segs[f].length;
         zb_skip_skippable(s, n);
         ZbHdr h; zb_parse_header(s, n, h);
-        ZbFrameInfo fi; fi.content_size = h.content_size; fi.dict_id = h.dict_id; fi.flags = h.checksum; fi.status = ZB_OK;
+        ZbFrameInfo fi; fi.content_size = h.content_size; fi.dict_id = h.dict_id; fi.flags = zb_info_flags(h); fi.status = ZB_OK;
         u64 pos = h.hdr_size, n_lit = 0, n_seq_rec = 0, n_blocks = 0;
         u32 err = ZB_OK; bool last = false;
         while (!last && !err) {
@@ -211,7 +214,7 @@ __global__ void zb_scan_frames(const u8* __restrict__ src, const ZbSegment* __re
     // whose header has no content size (zstd/zstd.c:45406-45453, ZSTD_d_windowLogMax / ZSTD_DCtx_setMaxWindowSize :45025)
     if (h.status == ZB_OK && h.content_size == ZB_CONTENT_UNKNOWN && h.window > window_limit) h.status = ZB_E_WINDOW_TOO_LARGE;
     if (h.status != ZB_OK) { fi.status = h.status; info[f] = fi; return; }
-    fi.content_size = h.content_size; fi.dict_id = h.dict_id; fi.flags = h.checksum;
+    fi.content_size = h.content_size; fi.dict_id = h.dict_id; fi.flags = zb_info_flags(h);
     if (big_list && n > ZB_SCAN_BIG) { big_list[1 + atomicAdd(big_list, 1u)] = f; return; }      // a warp's work: zb_scan_frames_big
     u64 pos = h.hdr_size;
     for (;;) {
@@ -313,7 +316,7 @@ zb_place_scan(const ZbFrameInfo* __restrict__ info, const u64* __restrict__ dst_
     }
     u32 const f = blockIdx.x * ZB_PLACE_CTA + tid;
     u64 v[4] = {0, 0, 0, 0}; u64 cap = 0; u32 st = ZB_OK;
-    if (f < n_frames) { ZbFrameInfo const fi = info[f]; zb_place_values(fi, dst_sizes, f, v, cap, st); status[f] = st; if ((fi.flags & 1) && st == ZB_OK) totals[4] = 1; }
+    if (f < n_frames) { ZbFrameInfo const fi = info[f]; zb_place_values(fi, dst_sizes, f, v, cap, st); status[f] = st; if ((fi.flags & 1) && st == ZB_OK) totals[4] = 1; if ((fi.flags & 2) && st == ZB_OK) totals[5] = 1; }
     u64 incl[4];
     #pragma unroll
     for (int k = 0; k < 4; k++) {

@@ -348,6 +348,9 @@ __device__ __forceinline__ u32 zb_seq_block(const u8* smem, u8* q, u8* ws, ZbDic
         // (a branch-free select chain over {rep0, rep1, rep2, rep0 - 1, new} was measured 3-5 % slower than this branch)
         if (ofc > 1) {
             off = (1u << ofc) - 3 + ob;
+            // SYMREP: bit 31 tags a symbolic history entry, so a concrete offset must stay below 2^31.  The launcher keeps
+            // frames whose window (plus the dictionary) reaches that far off the block path; here such an offset is corrupt.
+            if (SYMREP && (off & 0x80000000u)) { err = ZB_E_CORRUPTION; break; }
             rep2 = rep1; rep1 = rep0; rep0 = off;
         } else {
             u32 const ll0 = (llc == 0);
@@ -357,6 +360,8 @@ __device__ __forceinline__ u32 zb_seq_block(const u8* smem, u8* q, u8* ws, ZbDic
                 u32 const idx = 1 + ll0 + ob;
                 u32 const r0m = SYMREP && (rep0 & 0x80000000u) ? rep0 + 1 : rep0 - 1;   // symbolic: one more off
                 u32 tmp = idx == 1 ? rep1 : (idx == 2 ? rep2 : r0m);
+                // rep0 - 1 == 0 is corrupt (zstd/zstd.c:46905).  SYMREP rejects it here: 0xFFFFFFFF would read as symbolic.
+                if (SYMREP && tmp == 0) { err = ZB_E_CORRUPTION; break; }
                 if (tmp == 0) tmp = 0xFFFFFFFFu;
                 if (idx != 1) rep2 = rep1;
                 rep1 = rep0; rep0 = off = tmp;

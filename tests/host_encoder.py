@@ -293,6 +293,19 @@ DSIM_WRAPPERS = r"""
 // checksum verification, finish.  Output: tightly packed bytes + per-frame {offset, length}, status[] per frame.
 static int g_block_path = 0;
 extern "C" void t_set_block_path(int on) { g_block_path = on; }
+// The frame scans (small frames a thread each, big ones a warp each) and the placement, as zb_api.cu runs them before it
+// chooses a path: totals_out[0..5] = output, blocks, sequences, literals, any checksum, any window >= ZB_FAR_WINDOW.
+extern "C" void t_scan_totals(const u8* src, const u64* seg_off, const u64* seg_len, u32 n, u64* totals_out)
+{
+    std::vector<ZbSegment> segs(n); for (u32 i = 0; i < n; i++) { segs[i].offset = seg_off[i]; segs[i].length = seg_len[i]; }
+    std::vector<ZbFrameInfo> info(n); std::vector<ZbFramePlace> place(n + 1); std::vector<u32> status(n, 0), big(n + 1, 0);
+    u64 totals[8] = {0}; u32 const pctas = (n + ZB_PLACE_CTA - 1) / ZB_PLACE_CTA; std::vector<u64> partial(pctas * 4 + 4);
+    simt::launch((n + 127) / 128, 128, [&] { zb_scan_frames(src, segs.data(), n, info.data(), (1ull << 27) + 1, big.data()); });
+    simt::launch(n < 128 ? (n + 3) / 4 : 32, 128, [&] { zb_scan_frames_big(src, segs.data(), big.data(), info.data()); });
+    simt::launch(pctas, ZB_PLACE_CTA, [&] { zb_place_reduce(info.data(), nullptr, n, partial.data()); });
+    simt::launch(pctas, ZB_PLACE_CTA, [&] { zb_place_scan(info.data(), nullptr, n, partial.data(), place.data(), totals, status.data()); });
+    for (int k = 0; k < 6; k++) totals_out[k] = totals[k];
+}
 extern "C" long long t_decompress_batch(const u8* src, const u64* seg_off, const u64* seg_len, u32 n, const u8* dict_raw, u32 dict_n,
                                         u32 n_ctas, u32 warps, u32 take, u8* out, u64 out_cap, u64* out_off, u64* out_len, u32* status_out,
                                         const u64* dst_sizes /* nullable: the decompressed_sizes argument of the batch call */)
@@ -380,6 +393,8 @@ def build_decode_sim():
     L.t_decompress_batch.restype = C.c_longlong
     L.t_decompress_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32,
                                      C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.t_scan_totals.restype = None
+    L.t_scan_totals.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
     return L
 
 

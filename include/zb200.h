@@ -163,6 +163,25 @@ int zb200_compress_batch_ptrs(zb200_ctx* ctx, const void* const* srcs, const siz
 /* ZSTD_compressBound (zstd/zstd.c:4547) */
 uint64_t zb200_compress_bound(uint64_t src_size);
 
+/* ---- dictionary training: zstandard.train_dictionary (c-ext/compressiondict.c:13-146), which runs
+ * ZDICT_optimizeTrainFromBuffer_fastCover (zstd/zstd.c:52408).  Fields left at 0 take ZDICT's defaults or search ranges:
+ * d in {6, 8}, k in 50..2000 over `steps` (40) steps, f 20, accel 1, split_point 0.75, level 3, an ID derived from the
+ * content.  The caller applies train_dictionary's own defaulting (d 8, steps 4, level 3 when steps and threads are 0).
+ * The samples (host memory, packed back to back, sizes[i] bytes each) are uploaded once; hashing, counting, segment
+ * selection and finalisation of every candidate run on the device, each candidate is scored by compressing the test
+ * samples with it (zb200_compress_batch on the uploaded buffer), and the winner is copied to `out` (capacity bytes).
+ * Returns 0, a positive zstd error code when training fails as the reference's would (its name through
+ * zb200_ctx_last_error), or a negative value for an infrastructure failure. */
+typedef struct {
+    uint32_t k, d, f, steps, accel;
+    int32_t  level;               /* level of the candidate score's compression, 0 = 3 */
+    uint32_t dict_id;             /* 0 = XXH64 of the content, as ZDICT_finalizeDictionary */
+    uint32_t reserved;
+    double   split_point;         /* fraction of the samples trained on; the rest score the candidates. 0 = 0.75, 1 = all both */
+} zb200_train_params;
+int zb200_train_dictionary(zb200_ctx* ctx, const void* samples, const size_t* sizes, size_t n, const zb200_train_params* params,
+                           void* out, size_t capacity, size_t* out_size, uint32_t* chosen_k, uint32_t* chosen_d);
+
 /* ---- result accessors */
 const void*          zb200_result_data(const zb200_result* r);       /* host (pinned) or device pointer */
 uint64_t             zb200_result_size(const zb200_result* r);       /* bytes in data */

@@ -6,7 +6,7 @@ buffer types) so a caller can ``import python_zstandard_b200 as zstandard``:
     ZstdCompressor(...).multi_compress_to_buffer / .compress
     ZstdDecompressor(...).multi_decompress_to_buffer / .decompress
     BufferWithSegments, BufferSegments, BufferSegment, BufferWithSegmentsCollection
-    ZstdCompressionDict, ZstdError, frame helpers and constants
+    ZstdCompressionDict, train_dictionary (fastCover on the device), ZstdError, frame helpers and constants
     DeviceBufferWithSegments (not in the reference): the same batch calls on device-resident data, device-resident results
 
 All codec work runs as CUDA kernels in ``libzb200.so`` (C ABI: include/zb200.h).
@@ -15,7 +15,7 @@ from .errors import ZstdError  # noqa: F401
 from .buffers import (BufferSegment, BufferSegments, BufferWithSegments,  # noqa: F401
                       BufferWithSegmentsCollection, DeviceBufferWithSegments, DeviceBufferSegment)
 from .dictionary import (ZstdCompressionDict, DICT_TYPE_AUTO, DICT_TYPE_RAWCONTENT,  # noqa: F401
-                         DICT_TYPE_FULLDICT)
+                         DICT_TYPE_FULLDICT, train_dictionary)
 from .decompressor import ZstdDecompressor, FORMAT_ZSTD1, FORMAT_ZSTD1_MAGICLESS  # noqa: F401
 from .compressor import ZstdCompressor, ZstdCompressionParameters  # noqa: F401
 from ._native import set_device, default_device  # noqa: F401

@@ -30,6 +30,12 @@ class DParams(C.Structure):
     _fields_ = [("max_window_size", C.c_uint64), ("reserved", C.c_uint32 * 2)]
 
 
+class TrainParams(C.Structure):
+    """zb200_train_params (include/zb200.h)."""
+    _fields_ = [("k", C.c_uint32), ("d", C.c_uint32), ("f", C.c_uint32), ("steps", C.c_uint32), ("accel", C.c_uint32),
+                ("level", C.c_int32), ("dict_id", C.c_uint32), ("reserved", C.c_uint32), ("split_point", C.c_double)]
+
+
 class NativeError(RuntimeError):
     pass
 
@@ -95,6 +101,7 @@ def lib():
             "zb200_compress_batch_multi": (i, [vp, i, vp, vp, sz, vp, vp, sz, u32, vp, vp]),
             "zb200_multi_last_error": (C.c_char_p, []),
             "zb200_last_compress_kernel": (C.c_char_p, [vp]),
+            "zb200_train_dictionary": (i, [vp, vp, vp, sz, vp, vp, sz, C.POINTER(sz), C.POINTER(u32), C.POINTER(u32)]),
         }
         for name, (res, args) in sigs.items():
             f = getattr(L, name, None)

@@ -7,6 +7,8 @@
 // first-error selection.
 #include "zb_common.cuh"
 #include "../../include/zb200.h"
+#define ZT_TYPES_ONLY
+#include "zb_train.cuh"
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -55,7 +57,8 @@ void zb_launch_digest_dict(const u8* dict, u32 n, ZbDictDigest* out, cudaStream_
 size_t zb_encode_scratch_bytes();
 void zb_launch_compress_blocks(const u8* src, const void* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes,
                                void* outs, u32* work_counter, const u8* dict_tail, u32 dict_D, const u16* dict_table, const void* dict_digest, const void* dict_cct,
-                               const unsigned long long* upload_progress, unsigned long long upload_total, u32* upload_status, int dual, int small_blocks, cudaStream_t st);
+                               const unsigned long long* upload_progress, unsigned long long upload_total, u32* upload_status, int dual, int small_blocks, cudaStream_t st,
+                               u32* stats = nullptr);
 u32 zb_encode_small_max();
 void zb_launch_dict_table(const u8* tail, u32 D, u16* table, cudaStream_t st);
 u32 zb_encode_ctable_bytes();
@@ -73,6 +76,14 @@ void zb_launch_compress_recs(const u8* src, const void* jobs, u32 n_jobs, u32 n_
 size_t zb_encode2_scratch_bytes();
 void zb_launch_compress_smem(const u8* src, const void* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes, void* outs, u32* work_counter,
                              const unsigned long long* upload_progress, unsigned long long upload_total, u32* upload_status, cudaStream_t st);
+// dictionary training (zb_train.cuh)
+void zt_launch_hash(const u8* s, u32 n_dmers, u32 f, u32 d, u32* hash, u32 sms, cudaStream_t st);
+void zt_launch_count(const u32* hash, const u64* offs, u32 n_train, u32 step, u32* freqs, u32 sms, cudaStream_t st);
+void zt_launch_prev(const u32* hash, u32 n, u32* prev, u8* last, u32* table, cudaStream_t st);
+void zt_launch_select(const void* args, u32 n_ctas, cudaStream_t st);
+void zt_launch_entropy(const u32* stats, u32 content_size, u8* ent, u32* ent_len, cudaStream_t st);
+void zt_launch_finalize(const u8* dict, u32 cap, const u32* tail, const u8* ent, const u32* ent_len, u32 dict_id, u8* out, long long* res,
+                        cudaStream_t st);
 }
 
 namespace {
@@ -639,8 +650,10 @@ struct HostJob { u64 src_pos; u32 size, seg, last, first; };
 struct HostSegInfo { u64 first_job; u32 n_jobs, pad; };
 }
 
+// d_stats (dictionary training): u32[377] on the device that the block kernel's STATS instantiation adds its literal and
+// LL / ML / OF code counts to; only zb_compress_blocks has it, so such a call always runs that kernel
 static int compress_common(zb200_ctx* ctx, const void* src_base, const zb200_segment* segs, size_t n,
-                           const zb200_cparams* params, const zb200_ddict* dict, uint32_t flags, zb200_result** out)
+                           const zb200_cparams* params, const zb200_ddict* dict, uint32_t flags, zb200_result** out, u32* d_stats = nullptr)
 {
     *out = nullptr;
     if (!ctx || !segs || n == 0 || n > 0x7FFFFFF0u) return fail(ctx, "zb200_compress_batch: bad arguments", cudaSuccess);
@@ -699,10 +712,10 @@ static int compress_common(zb200_ctx* ctx, const void* src_base, const zb200_seg
     // Blocks of 8 KiB and more (no dictionary, level-3 class) take the round-2 kernel: one CTA per SM with the block resident in
     // shared memory.  Small blocks, dictionaries and the level >= 4 mode stay on the CTA-per-block kernel (6 CTAs per SM).
     static int const force_v1 = getenv("ZB200_ENCODER_V1") ? atoi(getenv("ZB200_ENCODER_V1")) : 0;
-    bool const smem_kernel = !dict && P.level < 4 && max_block >= 8192 && !force_v1;
+    bool const smem_kernel = !dict && P.level < 4 && max_block >= 8192 && !force_v1 && !d_stats;
     // Small records with a full dictionary (config 4): a warp per record, 22 records per SM (zb_encode3.cuh).
     bool const recs_kernel = dict && dict->c_D >= 8 && dict->dev.has_entropy && dict->d_cct && P.level < 4 && nj != 0 &&
-                             max_block <= zb_encode3_record_max() && !force_v1;
+                             max_block <= zb_encode3_record_max() && !force_v1 && !d_stats;
     u32 ctas = smem_kernel ? (u32)ctx->sm_count : (u32)ctx->sm_count * (227u * 1024u / zb_encode_smem_bytes());
     if (recs_kernel) { ctas = (u32)ctx->sm_count; u32 const need = ((u32)nj + zb_encode3_records_per_cta() - 1) / zb_encode3_records_per_cta(); if (ctas > need) ctas = need; }
     if (ctas > nj) ctas = (u32)nj;
@@ -753,7 +766,7 @@ static int compress_common(zb200_ctx* ctx, const void* src_base, const zb200_seg
       zb_launch_compress_blocks(d_src, ctx->jobs.p, (u32)nj, ctx->escratch.p, ctas, ctx->slots.as<u8>(), slot_bytes, ctx->bouts.p, d_counter,
                                 dict ? dict->c_tail : nullptr, dict ? dict->c_D : 0, dict ? dict->d_ctable : nullptr,
                                 (dict && dict->c_D && dict->dev.has_entropy) ? (const void*)dict->d_digest : nullptr, dict ? dict->d_cct : nullptr,
-                                overlap_upload ? d_progress : nullptr, up_bytes, d_upstatus, P.level >= 4 ? 1 : 0, max_block <= zb_encode_small_max() ? 1 : 0, ctx->stream); }
+                                overlap_upload ? d_progress : nullptr, up_bytes, d_upstatus, P.level >= 4 ? 1 : 0, max_block <= zb_encode_small_max() ? 1 : 0, ctx->stream, d_stats); }
     // the layout kernels read the input again (raw blocks): they wait for the whole upload, whatever order the segments came in
     if (overlap_upload) CK(cudaStreamWaitEvent(ctx->stream, ctx->chunk_ev[1], 0));
     { KSpan s(ctx, ZB200_K_LAYOUT);
@@ -977,3 +990,165 @@ int zb200_last_chase_rounds(const zb200_ctx* ctx) { return ctx->last_chase_round
 const char* zb200_last_compress_kernel(const zb200_ctx* ctx) { return ctx->last_compress_kernel; }
 
 }  // extern "C"
+
+// ---------------------------------------------------------------- dictionary training
+// zstandard.train_dictionary (c-ext/compressiondict.c:13-146) runs ZDICT_optimizeTrainFromBuffer_fastCover
+// (zstd/zstd.c:52408).  The samples go to the device once; hashing, counting, the previous-occurrence table, segment
+// selection and finalisation of every candidate run there (zb_train.cuh).  Each finished candidate comes back (at most
+// `capacity` bytes) to become a dictionary handle, and is scored by compressing the test samples -- still on the device --
+// with it: score = dictionary size + summed frame sizes (COVER_checkTotalCompressedSize, zstd/zstd.c:49352).  The smallest
+// score wins, ties go to the first candidate in ZDICT's loop order (d ascending, then k ascending).
+namespace {
+int train_fail(zb200_ctx* ctx, int code) { ctx->last_error = zb200_error_string(code); return code; }
+struct DevAllocs {
+    std::vector<void*> p;
+    ~DevAllocs() { for (void* q : p) cudaFree(q); }
+    template <class T> cudaError_t get(T** out, size_t bytes) { void* q = nullptr; cudaError_t e = cudaMalloc(&q, bytes ? bytes : 1); if (e == cudaSuccess) p.push_back(q); *out = (T*)q; return e; }
+};
+}  // namespace
+
+extern "C" int zb200_train_dictionary(zb200_ctx* ctx, const void* samples, const size_t* sizes, size_t n, const zb200_train_params* params,
+                                      void* out, size_t capacity, size_t* out_size, uint32_t* chosen_k, uint32_t* chosen_d)
+{
+    if (!ctx || !params || !out || !out_size || (n && (!samples || !sizes))) return fail(ctx, "zb200_train_dictionary: bad arguments", cudaSuccess);
+    cudaSetDevice(ctx->device);
+    zb200_train_params const P = *params;
+    // the parameter checks and the search range of ZDICT_optimizeTrainFromBuffer_fastCover, in its order
+    double const split = P.split_point <= 0.0 ? 0.75 : P.split_point;
+    u32 const min_d = P.d ? P.d : 6, max_d = P.d ? P.d : 8, min_k = P.k ? P.k : 50, max_k = P.k ? P.k : 2000;
+    u32 const steps = P.steps ? P.steps : 40, kstep = std::max((max_k - min_k) / steps, 1u);
+    u32 const f = P.f ? P.f : 20, accel = P.accel ? P.accel : 1;
+    if (split <= 0 || split > 1) return train_fail(ctx, 42);
+    if (accel == 0 || accel > 10) return train_fail(ctx, 42);
+    if (min_k < max_d || max_k < min_k) return train_fail(ctx, 42);
+    if (n == 0) return train_fail(ctx, 72);
+    if (capacity < 256) return train_fail(ctx, 70);
+    // FASTCOVER_ctx_init's checks (zstd/zstd.c:52103)
+    u32 const nb = (u32)n;
+    u32 const n_train = split < 1.0 ? (u32)((double)nb * split) : nb, n_test = split < 1.0 ? nb - n_train : nb;
+    std::vector<u64> offs(n + 1, 0);
+    for (size_t i = 0; i < n; i++) offs[i + 1] = offs[i] + sizes[i];
+    u64 const total = offs[n], train_size = offs[n_train];
+    if (total < std::max(min_d, 8u) || total >= 0xFFFFFFFFull || n_train < 5 || n_test < 1 || train_size < 8) return train_fail(ctx, 72);
+    u32 const n_dmers = (u32)(train_size - 8 + 1);
+    static const u32 fin_pct[11] = {100, 100, 50, 34, 25, 20, 17, 14, 13, 11, 10};      // FASTCOVER_defaultAccelParameters
+    u32 const step = accel, n_fin = (u32)((u64)n_train * fin_pct[accel] / 100);       // skip = accel - 1
+    // candidates; those FASTCOVER_checkParameters refuses are skipped, as there
+    std::vector<ZtCand> cands; u32 max_esz = 1;
+    for (u32 d = min_d; d <= max_d; d += 2)
+        for (u32 k = min_k; k <= max_k; k += kstep) {
+            if ((d == 6 || d == 8) && k <= capacity && d <= k && f >= 1 && f <= 31) {
+                cands.push_back(ZtCand{k, d, (d - min_d) / 2, 0});
+                u32 num, esz; zt_epochs((u32)capacity, n_dmers, k, num, esz); max_esz = std::max(max_esz, esz);
+            }
+            if (k > 0xFFFFFFFFu - kstep) break;
+        }
+    if (cands.empty()) return train_fail(ctx, 1);        // no candidate ran: COVER_best_t's initial (size_t)-1
+    u32 const cap = (u32)capacity;
+    size_t const tbl = (size_t)4 << f;
+    DevAllocs A;
+    u8* d_s; u64* d_offs; ZtCand* d_cand; u32 *d_tail, *d_stats, *d_entlen; u8* d_ent; long long* d_res;
+    CK(A.get(&d_s, total + 16)); CK(A.get(&d_offs, (n + 1) * 8)); CK(A.get(&d_cand, cands.size() * sizeof(ZtCand)));
+    CK(A.get(&d_tail, cands.size() * 4)); CK(A.get(&d_res, cands.size() * 8)); CK(A.get(&d_stats, 512 * 4)); CK(A.get(&d_ent, 512)); CK(A.get(&d_entlen, 4));
+    CK(cudaMemcpyAsync(d_s, samples, total, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemsetAsync(d_s + total, 0, 16, ctx->stream));
+    CK(cudaMemcpyAsync(d_offs, offs.data(), (n + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(d_cand, cands.data(), cands.size() * sizeof(ZtCand), cudaMemcpyHostToDevice, ctx->stream));
+    ZtSelect S; memset(&S, 0, sizeof S);
+    S.samples = d_s; S.cap = cap; S.tail = d_tail; S.cand = d_cand;
+    u32* d_freqs[2] = {nullptr, nullptr};
+    {   u8* d_last; u32* d_table;
+        CK(A.get(&d_last, n_dmers)); CK(A.get(&d_table, tbl));
+        for (u32 di = 0; di <= (max_d - min_d) / 2; di++) {
+            u32 const d = min_d + 2 * di;
+            if (d != 6 && d != 8) continue;
+            u32 *h, *pv;
+            CK(A.get(&h, (size_t)n_dmers * 4)); CK(A.get(&pv, (size_t)n_dmers * 4)); CK(A.get(&d_freqs[di], tbl));
+            zt_launch_hash(d_s, n_dmers, f, d, h, (u32)ctx->sm_count, ctx->stream); CK(cudaGetLastError());
+            CK(cudaMemsetAsync(d_freqs[di], 0, tbl, ctx->stream));
+            zt_launch_count(h, d_offs, n_train, step, d_freqs[di], (u32)ctx->sm_count, ctx->stream); CK(cudaGetLastError());
+            CK(cudaMemsetAsync(d_table, 0xFF, tbl, ctx->stream));
+            zt_launch_prev(h, n_dmers, pv, d_last, d_table, ctx->stream); CK(cudaGetLastError());
+            S.n_dmers[di] = n_dmers; S.hash[di] = h; S.prev[di] = pv;
+        }
+    }
+    CK(cudaStreamSynchronize(ctx->stream));
+    // candidates side by side, in waves that fit the free device memory
+    size_t const per = tbl + (size_t)4 * (max_esz + 2) + 2 * (size_t)cap;
+    size_t free_b = 0, total_b = 0; CK(cudaMemGetInfo(&free_b, &total_b));
+    size_t wave = std::min(cands.size(), std::max((size_t)1, free_b / 2 / per));
+    wave = std::min(wave, (size_t)ctx->sm_count * 2);
+    u32 *d_wfreqs, *d_diff; u8 *d_dict, *d_out;
+    CK(A.get(&d_wfreqs, wave * tbl)); CK(A.get(&d_diff, wave * 4 * (size_t)(max_esz + 2)));
+    CK(A.get(&d_dict, wave * (size_t)cap)); CK(A.get(&d_out, wave * (size_t)cap));
+    S.freqs = d_wfreqs; S.freqs_stride = tbl / 4; S.diff = d_diff; S.diff_stride = max_esz + 2; S.dict = d_dict;
+    // test samples: compressed where they lie, in the uploaded buffer
+    std::vector<zb200_segment> tsegs, fsegs;
+    for (u32 i = split < 1.0 ? n_train : 0; i < nb; i++) tsegs.push_back(zb200_segment{offs[i], sizes[i]});
+    // finalisation samples (ZDICT_countEStats): the first n_fin training samples, each cut to one 128 KiB block
+    for (u32 i = 0; i < n_fin; i++) fsegs.push_back(zb200_segment{offs[i], std::min<u64>(sizes[i], 128u << 10)});
+    int const level = P.level ? P.level : 3;
+    std::vector<u32> tails(cands.size());
+    std::vector<u8> host(wave * (size_t)cap), best;
+    std::vector<long long> res(cands.size());
+    u64 best_score = ~0ull; size_t best_c = 0;
+    for (size_t w0 = 0; w0 < cands.size(); w0 += wave) {
+        u32 const nw = (u32)std::min(wave, cands.size() - w0);
+        for (u32 i = 0; i < nw; i++)
+            CK(cudaMemcpyAsync(d_wfreqs + i * (tbl / 4), d_freqs[cands[w0 + i].di], tbl, cudaMemcpyDeviceToDevice, ctx->stream));
+        S.first = (u32)w0;
+        zt_launch_select(&S, nw, ctx->stream); CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(tails.data() + w0, d_tail + w0, nw * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaMemcpyAsync(host.data(), d_dict, (size_t)nw * cap, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        for (u32 i = 0; i < nw; i++) {
+            size_t const c = w0 + i;
+            // entropy statistics: the finalisation samples compressed with the candidate's content as a raw dictionary
+            u32 const csize = cap - tails[c];
+            zb200_ddict* raw = nullptr;
+            if (csize) { int rc = zb200_ddict_create(ctx, host.data() + (size_t)i * cap + tails[c], csize, &raw); if (rc) return rc < 0 ? rc : -1; }
+            CK(cudaMemsetAsync(d_stats, 0, 512 * 4, ctx->stream));
+            if (!fsegs.empty()) {
+                zb200_cparams cp; memset(&cp, 0, sizeof cp); cp.level = level; cp.write_content_size = 1;
+                zb200_result* r = nullptr;
+                int const rc = compress_common(ctx, d_s, fsegs.data(), fsegs.size(), &cp, raw, ZB200_SRC_DEVICE | ZB200_SEGS_HOST | ZB200_DST_DEVICE, &r, d_stats);
+                zb200_result_free(r);
+                if (rc) { zb200_ddict_free(raw); return rc; }
+            }
+            zb200_ddict_free(raw);
+            zt_launch_entropy(d_stats, csize, d_ent, d_entlen, ctx->stream); CK(cudaGetLastError());
+            zt_launch_finalize(d_dict + (size_t)i * cap, cap, d_tail + c, d_ent, d_entlen, P.dict_id, d_out + (size_t)i * cap, d_res + c, ctx->stream);
+            CK(cudaGetLastError());
+            CK(cudaMemcpyAsync(res.data() + c, d_res + c, 8, cudaMemcpyDeviceToHost, ctx->stream));
+            CK(cudaMemcpyAsync(host.data() + (size_t)i * cap, d_out + (size_t)i * cap, cap, cudaMemcpyDeviceToHost, ctx->stream));
+            CK(cudaStreamSynchronize(ctx->stream));
+            u64 score;
+            if (res[c] < 0) score = (u64)res[c];                       // (size_t)-code, as ZSTD errors compare in COVER_best_finish
+            else {
+                const u8* const dict = host.data() + (size_t)i * cap;
+                zb200_ddict* dd = nullptr;
+                int rc = zb200_ddict_create(ctx, dict, (size_t)res[c], &dd);
+                if (rc > 0 || rc == -1) return rc ? rc : -1;
+                if (rc < 0) score = (u64)(long long)rc;                // the digest refused the dictionary: its zstd code
+                else {
+                    zb200_cparams cp; memset(&cp, 0, sizeof cp);
+                    cp.level = P.level ? P.level : 3; cp.write_content_size = 1; cp.dict_id = zb200_ddict_id(dd);
+                    zb200_result* r = nullptr;
+                    rc = compress_common(ctx, d_s, tsegs.data(), tsegs.size(), &cp, dd, ZB200_SRC_DEVICE | ZB200_SEGS_HOST | ZB200_DST_DEVICE, &r);
+                    zb200_ddict_free(dd);
+                    if (rc) return rc;
+                    int code = 0;
+                    score = zb200_result_first_error(r, nullptr, &code, nullptr, nullptr) ? (u64)-(long long)code : (u64)res[c] + zb200_result_size(r);
+                    zb200_result_free(r);
+                }
+            }
+            if (score < best_score) { best_score = score; best_c = c; best.assign(host.data() + (size_t)i * cap, host.data() + (size_t)i * cap + (res[c] > 0 ? res[c] : 0)); }
+        }
+    }
+    if (best_score > ~0ull - 120) return train_fail(ctx, (int)(0 - best_score));      // ZSTD_isError: every candidate failed
+    memcpy(out, best.data(), best.size());
+    *out_size = best.size();
+    if (chosen_k) *chosen_k = cands[best_c].k;
+    if (chosen_d) *chosen_d = cands[best_c].d;
+    return 0;
+}

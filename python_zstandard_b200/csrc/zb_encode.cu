@@ -530,11 +530,14 @@ __device__ __forceinline__ u32 ze_off_code(u32 off, u32 ll, u32& r0, u32& r1, u3
 // bytes plus 2^13 heads keyed on 8 bytes; a position takes its 8-byte candidate when that one verifies 8 bytes.  CPU
 // model tools/enc_model3.c: 128 KiB text +3.2 % -> -1.6 % against level 3.  Used for level >= 4; the default
 // instantiation compiles to the code it had before.
-template <bool DUAL, u32 UNIT>
+// STATS (dictionary training only): every block coded as a compressed block adds its literal bytes and its LL / ML / OF code
+// histograms to stats[0..256), [256..292), [292..345), [345..377) -- the counts ZDICT_countEStats (zstd/zstd.c:53124) takes.
+// The pointer is null and unused in the other instantiations.
+template <bool DUAL, u32 UNIT, bool STATS = false>
 __global__ void __launch_bounds__(ZE_THREADS)
 zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jobs, u32 n_jobs,
                    ZeScratch* __restrict__ scratch, u8* __restrict__ slots, u64 slot_bytes,
-                   ZeBlockOut* __restrict__ outs, u32* __restrict__ work_counter, ZeDict dict, ZeUpload up)
+                   ZeBlockOut* __restrict__ outs, u32* __restrict__ work_counter, ZeDict dict, ZeUpload up, u32* __restrict__ stats = nullptr)
 {
     extern __shared__ __align__(16) u8 ze_smem_raw[];
     ZeShared& S = *(ZeShared*)ze_smem_raw;
@@ -1185,6 +1188,14 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
             outs[j].csize = 3 + S.body;
         }
         __syncthreads();
+        if constexpr (STATS) {
+            if (!S.use_raw) {
+                for (u32 i = tid; i < 256; i += ZE_THREADS) if (S.hist[i]) atomicAdd(&stats[i], S.hist[i]);
+                for (u32 i = tid; i < 36; i += ZE_THREADS) if (S.hLL[i]) atomicAdd(&stats[256 + i], S.hLL[i]);
+                for (u32 i = tid; i < 53; i += ZE_THREADS) if (S.hML[i]) atomicAdd(&stats[292 + i], S.hML[i]);
+                for (u32 i = tid; i < 32; i += ZE_THREADS) if (S.hOF[i]) atomicAdd(&stats[345 + i], S.hOF[i]);
+            }
+        }
         {
             u8* const o = out + 3;
             if (S.use_raw) { for (u32 i = tid; i < n; i += ZE_THREADS) o[i] = in[i]; }
@@ -1385,16 +1396,21 @@ void zb_launch_dict_table(const u8* tail, u32 D, u16* table, cudaStream_t st) { 
 
 void zb_launch_compress_blocks(const u8* src, const void* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes,
                                void* outs, u32* work_counter, const u8* dict_tail, u32 dict_D, const u16* dict_table, const void* dict_digest, const void* dict_cct,
-                               const unsigned long long* upload_progress, unsigned long long upload_total, u32* upload_status, int dual, int small_blocks, cudaStream_t st)
+                               const unsigned long long* upload_progress, unsigned long long upload_total, u32* upload_status, int dual, int small_blocks, cudaStream_t st,
+                               u32* stats)
 {
     ZeDict dict; dict.tail = dict_tail; dict.D = dict_D; dict.pad = 0; dict.table = dict_table; dict.ent = (const ZbDictDigest*)dict_digest; dict.cct = dict_digest ? dict_cct : nullptr;
     ZeUpload up; up.progress = upload_progress; up.total = upload_total; up.status = upload_status;
-    #define ZE_LAUNCH(D_, U_) do { \
-        cudaFuncSetAttribute(zb_compress_blocks<D_, U_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ZeShared));   /* per device: cheap, so set on every launch */ \
-        zb_compress_blocks<D_, U_><<<n_ctas, ZE_THREADS, sizeof(ZeShared), st>>>(src, (const ZeBlockJob*)jobs, n_jobs, (ZeScratch*)scratch, slots, slot_bytes, \
-                                                                                 (ZeBlockOut*)outs, work_counter, dict, up); } while (0)
-    if (dual) { if (small_blocks) ZE_LAUNCH(true, ZE_UNIT_SMALL); else ZE_LAUNCH(true, ZE_UNIT); }
-    else      { if (small_blocks) ZE_LAUNCH(false, ZE_UNIT_SMALL); else ZE_LAUNCH(false, ZE_UNIT); }
+    #define ZE_LAUNCH(D_, U_, S_) do { \
+        cudaFuncSetAttribute(zb_compress_blocks<D_, U_, S_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ZeShared));   /* per device: cheap, so set on every launch */ \
+        zb_compress_blocks<D_, U_, S_><<<n_ctas, ZE_THREADS, sizeof(ZeShared), st>>>(src, (const ZeBlockJob*)jobs, n_jobs, (ZeScratch*)scratch, slots, slot_bytes, \
+                                                                                     (ZeBlockOut*)outs, work_counter, dict, up, stats); } while (0)
+    if (stats) {        // dictionary training: the statistics of ZDICT_countEStats
+        if (dual) { if (small_blocks) ZE_LAUNCH(true, ZE_UNIT_SMALL, true); else ZE_LAUNCH(true, ZE_UNIT, true); }
+        else      { if (small_blocks) ZE_LAUNCH(false, ZE_UNIT_SMALL, true); else ZE_LAUNCH(false, ZE_UNIT, true); }
+    }
+    else if (dual) { if (small_blocks) ZE_LAUNCH(true, ZE_UNIT_SMALL, false); else ZE_LAUNCH(true, ZE_UNIT, false); }
+    else           { if (small_blocks) ZE_LAUNCH(false, ZE_UNIT_SMALL, false); else ZE_LAUNCH(false, ZE_UNIT, false); }
     #undef ZE_LAUNCH
 }
 
@@ -1463,3 +1479,6 @@ void zb_encode2_phase_read(unsigned long long* out16, int reset)
 }
 
 }  // extern "C"
+
+// dictionary training: its kernels and launchers (they reuse the entropy helpers above)
+#include "zb_train.cuh"

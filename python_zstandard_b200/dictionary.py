@@ -1,8 +1,9 @@
-"""ZstdCompressionDict -- the dictionary object handed to (de)compressors.
+"""ZstdCompressionDict -- the dictionary object handed to (de)compressors -- and train_dictionary.
 
-Mirrors c-ext/compressiondict.c:164-348 for the *use* of a dictionary (bytes,
-dict_id(), as_bytes(), len()).  Training (ZDICT_*, c-ext/compressiondict.c:13-146)
-is out of scope: train with the reference and pass the bytes in.
+ZstdCompressionDict mirrors c-ext/compressiondict.c:164-348 for the *use* of a dictionary (bytes,
+dict_id(), as_bytes(), len()).  train_dictionary mirrors c-ext/compressiondict.c:13-146: the fastCover
+trainer (ZDICT_optimizeTrainFromBuffer_fastCover) runs on the device through zb200_train_dictionary,
+candidates side by side, each scored with this package's own compressor.
 """
 import struct
 import threading
@@ -72,3 +73,38 @@ class ZstdCompressionDict:
                 self._ddicts[ctx.device] = h
                 weakref.finalize(self, ctx.L.zb200_ddict_free, h)
         return h
+
+
+def train_dictionary(dict_size, samples, k=0, d=0, f=0, split_point=0.0, accel=0, notifications=0, dict_id=0, level=0,
+                     steps=0, threads=0):
+    """zstandard.train_dictionary (c-ext/compressiondict.c:13-146): a full dictionary of at most dict_size bytes trained
+    from `samples` (a list of bytes) with fastCover, on the device.  `threads` only matters for the defaulting rule below
+    and `notifications` not at all: the candidates of the search always run side by side on the GPU."""
+    import ctypes as C
+    if not isinstance(samples, list):
+        raise TypeError("train_dictionary() argument 2 must be list, not %s" % type(samples).__name__)
+    for s in samples:
+        if not isinstance(s, bytes):
+            raise ValueError("samples must be bytes")
+    if threads < 0:
+        import os
+        threads = os.cpu_count() or 1
+    if not steps and not threads:          # the defaults of ZDICT_trainFromBuffer, as the reference applies them
+        d = d or 8
+        steps = steps or 4
+        level = level or 3
+    p = _native.TrainParams(k=k, d=d, f=f, steps=steps, accel=accel, level=level, dict_id=dict_id, reserved=0,
+                            split_point=split_point)
+    blob = b"".join(samples)
+    sizes = (C.c_size_t * max(len(samples), 1))(*[len(s) for s in samples])
+    out = C.create_string_buffer(max(dict_size, 1))
+    n = C.c_size_t(0)
+    ck, cd = C.c_uint32(0), C.c_uint32(0)
+    ctx = _native.Context.get(_native.default_device())
+    with ctx.lock:
+        rc = ctx.L.zb200_train_dictionary(ctx.h, blob, sizes, len(samples), C.byref(p), out, dict_size, C.byref(n),
+                                          C.byref(ck), C.byref(cd))
+    if rc > 0:
+        raise ZstdError("cannot train dict: %s" % ctx.last_error())
+    ctx.check(rc, "zb200_train_dictionary")
+    return ZstdCompressionDict(out.raw[:n.value], DICT_TYPE_FULLDICT, k=ck.value, d=cd.value)

@@ -18,6 +18,7 @@
  *   zb200_*_batch_multi         the worker partition and pool of both functions above: `threads` workers over contiguous
  *                               ranges balanced by bytes   c-ext/compressor.c:1127,1183-1200; c-ext/decompressor.c:1237,1290-1305
  *   zb200_dparams               ZstdDecompressor(max_window_size=) -> ZSTD_DCtx_setMaxWindowSize   c-ext/decompressor.c:17-60
+ *   zb200_decompress_chain      ZstdDecompressor.decompress_content_dict_chain   c-ext/decompressor.c:620-890
  *   zb200_cparams.window_log    ZSTD_c_windowLog of ZstdCompressionParameters   c-ext/compressionparams.c:46
  *   zb200_host_copy             the write into the result PyBytes   c-ext/decompressor.c:283-352
  *   ZB200_SRC/DST_DEVICE, ZB200_SEGS_HOST, zb200_pointer_device: no counterpart (device-resident callers, SURVEY.md 8(f)-2)
@@ -122,6 +123,19 @@ int zb200_decompress_batch_ex(zb200_ctx* ctx, const void* src_base, const zb200_
 int zb200_decompress_batch_ptrs_ex(zb200_ctx* ctx, const void* const* srcs, const size_t* sizes, size_t n,
                                    const uint64_t* dst_sizes, const zb200_ddict* dict, const zb200_dparams* params,
                                    uint32_t flags, zb200_result** out);
+
+/* ---- content-dictionary chains: decompress_content_dict_chain.  srcs[k] (sizes[k] bytes, host memory) is chunk k, one zstd
+ * frame with its content size in the header; chunk k >= 1 is decoded with chunk k-1's fulltext as a raw-content prefix
+ * (ZSTD_DCtx_refPrefix_advanced(..., ZSTD_dct_rawContent)), chunk 0 with first_dict (or none).  On success *out holds one
+ * segment, the last fulltext.  A chunk that fails -- a header check (bad frame, no content size, a dictionary ID on a
+ * prefixed chunk, a content size, window or prefix + content size of 2 GiB - 128 MiB or more: code 16) or its decoding --
+ * is reported through zb200_result_first_error as (chunk, zstd code); the lowest failing chunk wins, and chunks behind the
+ * first header failure are not looked at.  A chunk that starts with a skippable frame has an empty fulltext.
+ * params: accepted for API parity; a chain frame always has a content size, and then the reference does not apply the limit.
+ * The chain is decoded in runs of consecutive chunks sized to free device memory (ZB200_CHAIN_RUN_BYTES overrides the
+ * budget, for tests); each run starts from the previous run's last fulltext. */
+int zb200_decompress_chain(zb200_ctx* ctx, const void* const* srcs, const size_t* sizes, size_t n,
+                           const zb200_ddict* first_dict, const zb200_dparams* params, zb200_result** out);
 
 /* ---- one batch over several devices: the `threads` argument of the reference's batch calls as a C entry point.
  * The items are cut into contiguous ranges balanced by input bytes -- the reference's static worker partition

@@ -81,6 +81,7 @@ def lib():
             "zb200_decompress_batch_ptrs": (i, [vp, vp, vp, sz, vp, vp, u32, C.POINTER(vp)]),
             "zb200_decompress_batch_ex": (i, [vp, vp, vp, sz, vp, vp, vp, u32, C.POINTER(vp)]),
             "zb200_decompress_batch_ptrs_ex": (i, [vp, vp, vp, sz, vp, vp, vp, u32, C.POINTER(vp)]),
+            "zb200_decompress_chain": (i, [vp, vp, vp, sz, vp, vp, C.POINTER(vp)]),
             "zb200_compress_batch": (i, [vp, vp, vp, sz, vp, vp, u32, C.POINTER(vp)]),
             "zb200_compress_batch_ptrs": (i, [vp, vp, vp, sz, vp, vp, u32, C.POINTER(vp)]),
             "zb200_compress_bound": (u64, [u64]),

@@ -31,7 +31,7 @@ void zb_launch_entropy_blocks(const u8* src, const void* bdesc, u32 n_blocks, Zb
                               ZbDictDev dict, u32* status, void* bexit, u32 take, cudaStream_t st);
 void zb_launch_resolve_blocks(const u8* src, const ZbSegment* segs, u32 n, const ZbFramePlace* place, const ZbFrameInfo* info, const u64* dst_sizes,
                               ZbBlock* blocks, const void* bdesc, const void* bexit, const u64* frame_end, u64 n_blocks, ZbSeq* seqs, ZbDictDev dict,
-                              u32* status, u64* out_sizes, u32* ck_expect, u32* entry_rep, cudaStream_t st);
+                              u32* status, u64* out_sizes, u32* ck_expect, u32* entry_rep, cudaStream_t st, int chain);
 size_t zb_blkdesc_bytes();
 size_t zb_blkexit_bytes();
 void zb_launch_place(const ZbFrameInfo* info, const u64* dst_sizes, u32 n, ZbFramePlace* place, u64* totals,
@@ -43,7 +43,7 @@ size_t zb_wave_bytes(u64 n_frames, u64 n_blocks);
 size_t zb_chase_bytes(u64 n_total);
 int zb_launch_execute_chase(const u8* src, const ZbFramePlace* place, const u32* status, const ZbBlock* blocks, const void* bdesc,
                             const ZbSeq* seqs, const u8* lits, u8* dst, u64 lo, u64 hi, u64 n_total, u64 blk_first, u64 blk_last,
-                            void* ptr_mem, u32* d_changed, u32 n_ctas, ZbDictDev dict, cudaStream_t st);
+                            void* ptr_mem, u32* d_changed, u32 n_ctas, ZbDictDev dict, cudaStream_t st, int chain);
 void zb_launch_execute_big(const u8* src, const ZbFramePlace* place, const u32* status, const ZbBlock* blocks, const void* bdesc,
                            const ZbSeq* seqs, const u8* lits, u8* dst, u32 first, u32 end, u64 blk_first, u64 blk_last,
                            u64 n_frames, u64 n_blocks, void* wave_mem, u32 n_ctas, ZbDictDev dict, cudaStream_t st);
@@ -53,6 +53,7 @@ void zb_launch_execute(const u8* src, const ZbFramePlace* place, const u32* stat
                        const ZbSeq* seqs, const u8* lits, u8* dst, u32 first, u32 end, ZbDictDev dict, cudaStream_t st);
 void zb_launch_finish(const ZbFramePlace* place, const u64* out_sizes, const u32* status, u32 n, ZbSegment* out_segs,
                       u32* first_error, cudaStream_t st);
+void zb_launch_chain_shift(ZbFramePlace* place, u32 n, u64 carry, cudaStream_t st);
 void zb_launch_digest_dict(const u8* dict, u32 n, ZbDictDigest* out, cudaStream_t st);
 size_t zb_encode_scratch_bytes();
 void zb_launch_compress_blocks(const u8* src, const void* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes,
@@ -121,6 +122,7 @@ struct zb200_ctx {
     DevBuf bdesc, bexit, erep, fend, wave;    // block-parallel decode path
     DevBuf biglist;                           // frames whose scans are a warp's work (zb_scan_frames_big)
     DevBuf chase;                             // its pointer-jumping execute stage: a source pointer per output byte
+    DevBuf carry;                             // content-dictionary chains: the last fulltext of a run, the prefix of the next
     int last_chase_rounds = 0;
     const char* last_compress_kernel = "";    // which of the three block kernels the last compress call ran (profile slot zb_compress_blocks)
     u32 entropy_warps = 0;
@@ -248,7 +250,7 @@ void zb200_ctx_destroy(zb200_ctx* ctx)
     if (!ctx) return;
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
-    ctx->bdesc.release(); ctx->bexit.release(); ctx->erep.release(); ctx->fend.release(); ctx->wave.release(); ctx->chase.release(); ctx->biglist.release();
+    ctx->bdesc.release(); ctx->bexit.release(); ctx->erep.release(); ctx->fend.release(); ctx->wave.release(); ctx->chase.release(); ctx->biglist.release(); ctx->carry.release();
     DevBuf* all[] = {&ctx->src, &ctx->segs, &ctx->dst_sizes, &ctx->info, &ctx->place, &ctx->status, &ctx->out_sizes,
                      &ctx->blocks, &ctx->seqs, &ctx->lits, &ctx->dst, &ctx->lane, &ctx->small, &ctx->out_segs, &ctx->partial,
                      &ctx->jobs, &ctx->seginfo, &ctx->slots, &ctx->bouts, &ctx->escratch, &ctx->fsizes, &ctx->ck};
@@ -395,8 +397,13 @@ uint32_t zb200_ddict_id(const zb200_ddict* d) { return d ? d->dev.dict_id : 0; }
 // ---------------------------------------------------------------- batch decompression
 // Device-side pipeline shared by the host and device entry points.  d_src/d_segs/d_dst_sizes are device
 // pointers.  On return the output is in ctx->dst (or caller_dst), segment table + status on the host.
+// chain: content-dictionary chain mode (zb200_decompress_chain).  The frames are revisions, each one's prefix is the previous
+// one's output; the carried prefix -- ctx->carry, chain->carry bytes -- goes in front of frame 0.  The output stays in ctx->dst
+// (nothing is copied back) and the path is always the block path with the pointer-jumping execute stage.
+struct ChainRun { u64 carry; };
 static int run_decompress(zb200_ctx* ctx, const u8* d_src, const ZbSegment* d_segs, size_t n, const u64* d_dst_sizes,
-                          const zb200_ddict* dict, zb200_result* res, bool copy_back, bool exact_sizes, u64 window_limit)
+                          const zb200_ddict* dict, zb200_result* res, bool copy_back, bool exact_sizes, u64 window_limit,
+                          const ChainRun* chain = nullptr)
 {
     u32 const nf = (u32)n;
     ZbDictDev dd = dict ? dict->dev : no_dict();
@@ -422,7 +429,12 @@ static int run_decompress(zb200_ctx* ctx, const u8* d_src, const ZbSegment* d_se
                       ctx->status.as<u32>(), ctx->partial.as<u64>(), ctx->stream); }
     u64 totals[6];          // output, blocks, sequences, literals, any checksum, any window >= ZB_FAR_WINDOW
     CK(cudaMemcpyAsync(totals, d_totals, sizeof totals, cudaMemcpyDeviceToHost, ctx->stream));
+    if (chain && chain->carry) zb_launch_chain_shift(ctx->place.as<ZbFramePlace>(), nf, chain->carry, ctx->stream);
     CK(cudaStreamSynchronize(ctx->stream));
+    if (chain) {
+        if (totals[5]) return fail(ctx, "zb200_decompress_chain: a window of ZB_FAR_WINDOW or more", cudaSuccess);
+        totals[0] += chain->carry;
+    }
 
     // persistent entropy grid: one CTA per SM (its shared memory holds the decode tables); trimmed per chunk below
     u32 const ctas = (u32)ctx->sm_count;
@@ -432,7 +444,10 @@ static int run_decompress(zb200_ctx* ctx, const u8* d_src, const ZbSegment* d_se
     // the output: the context's arena when it is copied back to the host, an allocation of its own (stream-ordered pool)
     // when the caller keeps it on the device -- the next call on this context must not touch a live result
     u8* d_out;
-    if (copy_back) { CK(ctx->dst.ensure(totals[0] + 64)); d_out = ctx->dst.as<u8>(); }
+    if (copy_back || chain) {
+        CK(ctx->dst.ensure(totals[0] + 64)); d_out = ctx->dst.as<u8>();
+        if (chain && chain->carry) CK(cudaMemcpyAsync(d_out, ctx->carry.p, chain->carry, cudaMemcpyDeviceToDevice, ctx->stream));
+    }
     else { void* p = nullptr; CK(cudaMallocAsync(&p, totals[0] + 64, ctx->stream)); d_out = (u8*)p; res->data = p; res->data_on_device = true; res->data_owned_device = true; }
     ctx->last_scratch = (totals[1] + 1) * sizeof(ZbBlock) + (totals[2] + 1) * sizeof(ZbSeq) + totals[3];
 
@@ -457,7 +472,7 @@ static int run_decompress(zb200_ctx* ctx, const u8* d_src, const ZbSegment* d_se
     // offset can reach 2^31: a frame with a window of ZB_FAR_WINDOW or more, or a dictionary of ZB_FAR_DICT bytes or more.
     int const force_blocks = getenv("ZB200_BLOCK_PATH") ? atoi(getenv("ZB200_BLOCK_PATH")) : -1;      // (read per call: tests switch it)
     bool const far = totals[5] != 0 || dd.content_size >= ZB_FAR_DICT;
-    bool const block_path = !far && (force_blocks >= 0 ? force_blocks != 0 : (totals[1] > n && n < 3000 && totals[0] >= (u64)n * (512u << 10)));
+    bool const block_path = chain || (!far && (force_blocks >= 0 ? force_blocks != 0 : (totals[1] > n && n < 3000 && totals[0] >= (u64)n * (512u << 10))));
     bool chase_path = false;
     ctx->last_chase_rounds = 0;
     if (block_path) {
@@ -470,8 +485,9 @@ static int run_decompress(zb200_ctx* ctx, const u8* d_src, const ZbSegment* d_se
         // FEW frames of many blocks (one huge frame at the limit): the copy-execute chain of a frame is serial however it is
         // mapped, so it is shortened by pointer doubling instead (zb_chase_*); many frames keep the machine busy frame-parallel
         int const force_chase = getenv("ZB200_CHASE") ? atoi(getenv("ZB200_CHASE")) : -1;
-        chase_path = force_chase >= 0 ? force_chase != 0 : (nf < 64 && nb >= 8ull * nf);
-        if (chase_path && ctx->chase.ensure(zb_chase_bytes(totals[0])) != cudaSuccess) { cudaGetLastError(); chase_path = false; }
+        chase_path = chain || (force_chase >= 0 ? force_chase != 0 : (nf < 64 && nb >= 8ull * nf));
+        if (chain) CK(ctx->chase.ensure(zb_chase_bytes(totals[0])));      // frames of a chain are not independent: no other execute
+        else if (chase_path && ctx->chase.ensure(zb_chase_bytes(totals[0])) != cudaSuccess) { cudaGetLastError(); chase_path = false; }
         { KSpan s(ctx, ZB200_K_SCAN);
           zb_launch_scan_blocks(d_src, d_segs, nf, ctx->place.as<ZbFramePlace>(), dd, ctx->status.as<u32>(), ctx->bdesc.p, ctx->fend.as<u64>(), ctx->biglist.as<u32>(), ctx->stream); }
         u32 const take = 3, EW = 7;
@@ -482,7 +498,7 @@ static int run_decompress(zb200_ctx* ctx, const u8* d_src, const ZbSegment* d_se
         { KSpan s(ctx, ZB200_K_PLACE);
           zb_launch_resolve_blocks(d_src, d_segs, nf, ctx->place.as<ZbFramePlace>(), ctx->info.as<ZbFrameInfo>(), exact_sizes ? d_dst_sizes : nullptr,
                                    ctx->blocks.as<ZbBlock>(), ctx->bdesc.p, ctx->bexit.p, ctx->fend.as<u64>(), nb, ctx->seqs.as<ZbSeq>(), dd,
-                                   ctx->status.as<u32>(), ctx->out_sizes.as<u64>(), ctx->ck.as<u32>(), ctx->erep.as<u32>(), ctx->stream); }
+                                   ctx->status.as<u32>(), ctx->out_sizes.as<u64>(), ctx->ck.as<u32>(), ctx->erep.as<u32>(), ctx->stream, chain != nullptr); }
     }
     res->n = n; res->size = totals[0];
     res->segs.resize(n);
@@ -511,7 +527,7 @@ static int run_decompress(zb200_ctx* ctx, const u8* d_src, const ZbSegment* d_se
                                                     ctx->seqs.as<ZbSeq>(), ctx->lits.as<u8>(), d_out,
                                                     n_chunks > 1 ? cpl[k].dst_off : 0, n_chunks > 1 ? cpl[k + 1].dst_off : totals[0], totals[0],
                                                     n_chunks > 1 ? cpl[k].blk_off : 0, n_chunks > 1 ? cpl[k + 1].blk_off : totals[1],
-                                                    ctx->chase.p, d_counter + 48, ctas, dd, ctx->stream);
+                                                    ctx->chase.p, d_counter + 48, ctas, dd, ctx->stream, chain != nullptr);
               if (r < 0) return fail(ctx, "pointer-jumping execute", cudaGetLastError());
               ctx->last_chase_rounds = r;
           }
@@ -641,6 +657,131 @@ int zb200_decompress_batch_ptrs_ex(zb200_ctx* ctx, const void* const* srcs, cons
     int rc = decompress_common(ctx, stage, segs.data(), n, dst_sizes, dict, flags & ~ZB200_SRC_DEVICE, out, params);
     pinned_put(ctx, stage);
     return rc;
+}
+
+// ---------------------------------------------------------------- content-dictionary chains
+// decompress_content_dict_chain (c-ext/decompressor.c:620-890): frame k is decoded with frame k-1's fulltext as a raw-content
+// prefix, and only the last fulltext is returned.  The entropy stage of every frame is independent (a raw-content prefix
+// brings no tables and no repcodes), so all frames of a run go through the block path side by side; only the LZ execute is
+// chained, and the pointer-jumping stage shortens those chains across frame borders instead of following them.
+// A run is as many consecutive frames as fit the memory budget; the next run starts from its last fulltext.
+int zb200_decompress_chain(zb200_ctx* ctx, const void* const* srcs, const size_t* sizes, size_t n,
+                           const zb200_ddict* first_dict, const zb200_dparams* params, zb200_result** out)
+{
+    *out = nullptr;
+    if (!ctx || !srcs || !sizes || n == 0 || n > 0x7FFFFFF0u) return fail(ctx, "zb200_decompress_chain: bad arguments", cudaSuccess);
+    cudaSetDevice(ctx->device);
+    // ---- the header checks, chunk by chunk; the first chunk that fails one ends the chain (h): chunks [0, h) are decoded,
+    // and a decode error among them wins, as when the reference decodes chunk k before it looks at chunk k + 1
+    std::vector<u64> csize(n, 0);
+    std::vector<char> skip(n, 0);
+    size_t h = n; int h_code = 0;
+    for (size_t k = 0; k < n && h == n; k++) {
+        const u8* s = (const u8*)srcs[k];
+        int code = 0;
+        if (sizes[k] >= 4 && (((u32)s[0] | (u32)s[1] << 8 | (u32)s[2] << 16 | (u32)s[3] << 24) & 0xFFFFFFF0u) == ZB_MAGIC_SKIP) {
+            // a skippable frame first: the reference's stream decoder stops behind it, so the fulltext is empty
+            u64 const len = sizes[k] >= 8 ? ((u32)s[4] | (u32)s[5] << 8 | (u32)s[6] << 16 | (u64)s[7] << 24) : 0;
+            if (sizes[k] < 8 + len) code = ZB_E_SRCSIZE_WRONG;
+            skip[k] = 1;
+        } else {
+            zb200_frame_info_t fi; zb200_frame_info(s, sizes[k], &fi);
+            if (fi.status) code = (int)fi.status;
+            else if (fi.content_size == ~0ull) code = ZB200_E_UNKNOWN_SIZE;
+            // the block path reads offsets of 2^31 and more as symbolic repcodes (DESIGN.md section 6); a match may reach
+            // back over the whole prefix, so the prefix counts too
+            else if (fi.content_size >= ZB_FAR_WINDOW || fi.window_size >= ZB_FAR_WINDOW
+                     || (k && csize[k - 1] + fi.content_size >= ZB_FAR_WINDOW)) code = ZB_E_WINDOW_TOO_LARGE;
+            // a raw-content prefix has dictionary ID 0, and zstd checks the header's ID against it (zstd/zstd.c:43938)
+            else if (fi.dict_id && !(k == 0 && first_dict)) code = ZB_E_DICT_WRONG;
+            else csize[k] = fi.content_size;
+        }
+        if (code) { h = k; h_code = code; }
+    }
+    zb200_result* res = new zb200_result(); res->ctx = ctx;
+    auto finish = [&](int rc) { if (rc) zb200_result_free(res); else *out = res; return rc; };
+    auto chunk_error = [&](size_t k, int code) { res->has_error = true; res->err_item = k; res->err_code = code; };
+    // ---- every chunk before h goes to the device once
+    u64 total = 0; for (size_t k = 0; k < h; k++) total += sizes[k];
+    std::vector<zb200_segment> segs(h);
+    if (h) {
+        u8* stage = (u8*)pinned_get(ctx, total ? total : 1);
+        if (!stage) return finish(fail(ctx, "pinned staging allocation", cudaErrorMemoryAllocation));
+        u64 pos = 0;
+        for (size_t k = 0; k < h; k++) { memcpy(stage + pos, srcs[k], sizes[k]); segs[k].offset = pos; segs[k].length = sizes[k]; pos += sizes[k]; }
+        cudaError_t e = ctx->src.ensure(total + 64);
+        if (e == cudaSuccess) e = ctx->segs.ensure(h * sizeof(ZbSegment));
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->src.p, stage, total, cudaMemcpyHostToDevice, ctx->stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->segs.p, segs.data(), h * sizeof(ZbSegment), cudaMemcpyHostToDevice, ctx->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+        pinned_put(ctx, stage);
+        if (e != cudaSuccess) return finish(fail(ctx, "zb200_decompress_chain upload", e));
+    }
+    const u8* const d_src = ctx->src.as<u8>(); const ZbSegment* const d_segs = ctx->segs.as<ZbSegment>();
+    u64 const wl = window_limit_of(params);
+    u64 carry = 0;              // bytes of the last fulltext in ctx->carry
+    size_t k = 0;
+    // ---- chunk 0 with the decompressor's dictionary: on its own through the batch path; its output is the first carry
+    if (h && first_dict && !skip[0]) {
+        zb200_result* r0 = new zb200_result(); r0->ctx = ctx;
+        int rc = run_decompress(ctx, d_src, d_segs, 1, nullptr, first_dict, r0, false, true, wl);
+        cudaError_t e = cudaSuccess;
+        if (!rc && !r0->has_error && csize[0]) {
+            e = ctx->carry.ensure(csize[0]);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->carry.p, r0->data, csize[0], cudaMemcpyDeviceToDevice, ctx->stream);
+        }
+        if (!rc && r0->has_error) chunk_error(0, r0->err_code);
+        zb200_result_free(r0);
+        if (rc) return finish(rc);
+        if (e != cudaSuccess) return finish(fail(ctx, "zb200_decompress_chain carry", e));
+        if (res->has_error) return finish(0);
+        carry = csize[0]; k = 1;
+    }
+    // ---- runs: device bytes per chunk of output ~ 1 (fulltext) + 8 (pointer) + 5.3 (sequence records of >= 3-byte matches)
+    // + 1 (literals); the budget is most of the free device memory, or ZB200_CHAIN_RUN_BYTES (read per call: tests force runs)
+    u64 budget;
+    {
+        const char* env = getenv("ZB200_CHAIN_RUN_BYTES");
+        size_t fr = 0, tot = 0; cudaMemGetInfo(&fr, &tot);
+        budget = env && *env ? strtoull(env, nullptr, 10) : (u64)fr / 10 * 6;
+    }
+    auto cost = [&](size_t j) { return 16 * csize[j] + sizes[j] + 4096; };
+    int rounds = 0;
+    while (k < h) {
+        if (skip[k]) { carry = 0; k++; continue; }
+        size_t b = k + 1; u64 use = 16 * carry + cost(k);
+        while (b < h && !skip[b] && use + cost(b) <= budget) use += cost(b++);
+        zb200_result* rr = new zb200_result(); rr->ctx = ctx;
+        ChainRun cr; cr.carry = carry;
+        int rc = run_decompress(ctx, d_src, d_segs + k, b - k, nullptr, nullptr, rr, false, true, wl, &cr);
+        rounds += ctx->last_chase_rounds;
+        cudaError_t e = cudaSuccess;
+        if (!rc && rr->has_error) chunk_error(k + rr->err_item, rr->err_code);
+        else if (!rc) {         // the run's last fulltext becomes the next prefix
+            zb200_segment const last = rr->segs[b - k - 1];
+            carry = last.length;
+            if (carry) e = ctx->carry.ensure(carry);
+            if (carry && e == cudaSuccess) e = cudaMemcpyAsync(ctx->carry.p, ctx->dst.as<u8>() + last.offset, carry, cudaMemcpyDeviceToDevice, ctx->stream);
+        }
+        zb200_result_free(rr);
+        if (rc) return finish(rc);
+        if (e != cudaSuccess) return finish(fail(ctx, "zb200_decompress_chain carry", e));
+        if (res->has_error) { ctx->last_chase_rounds = rounds; return finish(0); }
+        k = b;
+    }
+    ctx->last_chase_rounds = rounds;
+    if (h < n) { chunk_error(h, h_code); return finish(0); }
+    // ---- the last fulltext, copied back alone
+    res->data = pinned_get(ctx, carry ? carry : 1);
+    if (!res->data) return finish(fail(ctx, "pinned output allocation", cudaErrorMemoryAllocation));
+    res->data_pinned_pool = true;
+    if (carry) {
+        cudaError_t e = cudaMemcpyAsync(res->data, ctx->carry.p, carry, cudaMemcpyDeviceToHost, ctx->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+        if (e != cudaSuccess) return finish(fail(ctx, "zb200_decompress_chain copy-back", e));
+    }
+    res->n = 1; res->size = carry; res->segs.assign(1, zb200_segment{0, carry});
+    return finish(0);
 }
 
 

@@ -740,9 +740,12 @@ __global__ void zb_resolve_blocks(const u8* __restrict__ src, const ZbSegment* _
 
 // K3c: zb_patch_blocks -- a warp per block: symbolic offsets become distances, and every offset is checked against what
 // has been regenerated in front of it (the check of ZSTD_execSequence, zstd/zstd.c:46666, that zb_entropy_blocks postponed).
+// Chain mode (decompress_content_dict_chain): no dictionary; frame f may reach the bytes between its predecessor's start and
+// its own, place[f].dst_off - place[f - 1].dst_off (frame 0: the carried prefix, which the launcher put in front of it).
 __global__ void __launch_bounds__(256)
 zb_patch_blocks(const ZbBlock* __restrict__ blocks, const ZbBlkDesc* __restrict__ bdesc, u64 n_blocks, ZbSeq* __restrict__ seqs,
-                const u32* __restrict__ entry_rep, ZbDictDev dict, u32* __restrict__ status)
+                const u32* __restrict__ entry_rep, ZbDictDev dict, u32* __restrict__ status,
+                const ZbFramePlace* __restrict__ chain_place = nullptr)
 {
     u32 const lane = threadIdx.x & 31;
     u64 const b = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -751,6 +754,7 @@ zb_patch_blocks(const ZbBlock* __restrict__ blocks, const ZbBlkDesc* __restrict_
     if ((D.flags & ZB_BD_SKIP) || status[D.frame] != ZB_OK) return;
     ZbBlock const B = blocks[b];
     if (B.kind != ZB_BLK_COMPRESSED || B.n_seq == 0) return;
+    u64 const reach = chain_place ? chain_place[D.frame].dst_off - (D.frame ? chain_place[D.frame - 1].dst_off : 0) : dict.content_size;
     u32 const e0 = entry_rep[3 * b], e1 = entry_rep[3 * b + 1], e2 = entry_rep[3 * b + 2];
     ZbSeq* const sq = seqs + B.seq_pos;
     bool bad = false;
@@ -763,7 +767,7 @@ zb_patch_blocks(const ZbBlock* __restrict__ blocks, const ZbBlkDesc* __restrict_
             sq[i].w = r.w;
         }
         u64 const mstart = B.out_pos + r.y + (lit_next - r.x);            // frame-relative start of the match
-        if ((u64)r.w > mstart + dict.content_size) {
+        if ((u64)r.w > mstart + reach) {
             bad = true;
 #ifdef ZB_DEBUG_BLOCKS
             printf("[patch] block %llu seq %u off %u (raw %u) mstart %llu out_pos %llu e %u %u %u\n", (unsigned long long)b, i, r.w, sq[i].w, (unsigned long long)mstart,
@@ -1377,7 +1381,8 @@ template <typename P>
 __global__ void __launch_bounds__(256)
 zb_chase_init(const u8* __restrict__ src, const ZbFramePlace* __restrict__ place, const u32* __restrict__ status,
               const ZbBlock* __restrict__ blocks, const ZbBlkDesc* __restrict__ bdesc, const ZbSeq* __restrict__ seqs,
-              const u8* __restrict__ lits, u8* __restrict__ dst, P* __restrict__ ptr, u64 blk_first, u64 blk_last, ZbDictDev dict)
+              const u8* __restrict__ lits, u8* __restrict__ dst, P* __restrict__ ptr, u64 blk_first, u64 blk_last, ZbDictDev dict,
+              bool chain = false)
 {
     P const DONE = zb_chase_done<P>();
     u32 const tid = threadIdx.x, lane = tid & 31;
@@ -1396,7 +1401,9 @@ zb_chase_init(const u8* __restrict__ src, const ZbFramePlace* __restrict__ place
         const u8* const lit = B.lit_kind == ZB_LIT_RAW ? src + B.src_pos : lits + B.src_pos;
         const ZbSeq* const sq = seqs + B.seq_pos;
         u32 const nseq = B.n_seq;
-        long long const fstart = (long long)pl.dst_off;    // sources below it come from the dictionary
+        // sources below fstart come from the dictionary; in chain mode the previous frame's output (the carried prefix in
+        // front of frame 0) is part of dst, so they are pointed at like any other byte
+        long long const fstart = chain ? (f ? (long long)place[f - 1].dst_off : 0ll) : (long long)pl.dst_off;
         for (u32 g = 0; g < nseq; g += 256) {
             u32 const i = g + tid; bool const valid = i < nseq;
             ZbSeq r = make_uint4(0, 0, 0, 0); u32 nx = 0;
@@ -1427,6 +1434,15 @@ zb_chase_init(const u8* __restrict__ src, const ZbFramePlace* __restrict__ place
             for (u32 k = tid; k < tail; k += 256) { gout[e.y + k] = lit_rle ? lit_byte : lit[e.x + k]; gp[e.y + k] = (P)(gbase + e.y + k) | DONE; }
         }
     }
+}
+
+// chain mode: the carried prefix in front of frame 0 (place[0].dst_off bytes) is final; its bytes are their own sources
+template <typename P>
+__global__ void __launch_bounds__(256)
+zb_chase_prefix(const ZbFramePlace* __restrict__ place, P* __restrict__ ptr)
+{
+    u64 const carry = place[0].dst_off, stride = (u64)gridDim.x * 256;
+    for (u64 p = (u64)blockIdx.x * 256 + threadIdx.x; p < carry; p += stride) ptr[p] = (P)p | zb_chase_done<P>();
 }
 
 // one round of pointer doubling over [lo, hi).  Racing updates are harmless: whatever a thread reads from ptr[q] is an ancestor
@@ -1591,6 +1607,13 @@ __global__ void zb_finish(const ZbFramePlace* __restrict__ place, const u64* __r
     if (status[f] != ZB_OK) atomicMin(first_error, f);
 }
 
+// chain mode: the run's frames are placed behind the `carry` bytes of the prefix carried in from the previous run
+__global__ void zb_chain_shift(ZbFramePlace* __restrict__ place, u32 n_entries, u64 carry)
+{
+    u32 const i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n_entries) place[i].dst_off += carry;
+}
+
 // ===========================================================================
 // dictionary digest -- one thread, once per dictionary
 // (restates ZSTD_loadDEntropy zstd/zstd.c:44673-44757 and ZSTD_decompress_insertDictionary :44760)
@@ -1674,11 +1697,12 @@ void zb_launch_entropy_blocks(const u8* src, const void* bdesc, u32 n_blocks, Zb
 }
 void zb_launch_resolve_blocks(const u8* src, const ZbSegment* segs, u32 n, const ZbFramePlace* place, const ZbFrameInfo* info, const u64* dst_sizes,
                               ZbBlock* blocks, const void* bdesc, const void* bexit, const u64* frame_end, u64 n_blocks, ZbSeq* seqs, ZbDictDev dict,
-                              u32* status, u64* out_sizes, u32* ck_expect, u32* entry_rep, cudaStream_t st)
+                              u32* status, u64* out_sizes, u32* ck_expect, u32* entry_rep, cudaStream_t st, int chain)
 {
     zb_resolve_blocks<<<(n + 63) / 64, 64, 0, st>>>(src, segs, n, place, info, dst_sizes, blocks, (const ZbBlkDesc*)bdesc, (const ZbBlkExit*)bexit,
                                                    frame_end, dict, status, out_sizes, ck_expect, entry_rep);
-    if (n_blocks) zb_patch_blocks<<<(unsigned)((n_blocks + 7) / 8), 256, 0, st>>>(blocks, (const ZbBlkDesc*)bdesc, n_blocks, seqs, entry_rep, dict, status);
+    if (n_blocks) zb_patch_blocks<<<(unsigned)((n_blocks + 7) / 8), 256, 0, st>>>(blocks, (const ZbBlkDesc*)bdesc, n_blocks, seqs, entry_rep, dict, status,
+                                                                                    chain ? place : nullptr);
 }
 size_t zb_blkdesc_bytes() { return sizeof(ZbBlkDesc); }
 size_t zb_blkexit_bytes() { return sizeof(ZbBlkExit); }
@@ -1715,14 +1739,15 @@ extern "C++" {
 template <typename P>
 static int zb_chase_run(const u8* src, const ZbFramePlace* place, const u32* status, const ZbBlock* blocks, const void* bdesc,
                         const ZbSeq* seqs, const u8* lits, u8* dst, u64 lo, u64 hi, u64 n_total, u64 blk_first, u64 blk_last,
-                        void* ptr_mem, u32* d_changed, u32 n_ctas, ZbDictDev dict, cudaStream_t st)
+                        void* ptr_mem, u32* d_changed, u32 n_ctas, ZbDictDev dict, cudaStream_t st, bool chain)
 {
     P* const ptr = (P*)ptr_mem;
     if (hi <= lo || blk_last <= blk_first) return 0;
     if (cudaMemsetAsync(ptr + lo, 0xFF, (hi - lo) * sizeof(P), st) != cudaSuccess) return -1;      // frames that failed stay "done, no source"
     u64 const nb = blk_last - blk_first;
+    if (chain) zb_chase_prefix<P><<<n_ctas * 4, 256, 0, st>>>(place, ptr);
     zb_chase_init<P><<<(unsigned)(nb < n_ctas * 8ull ? nb : n_ctas * 8ull), 256, 0, st>>>(src, place, status, blocks, (const ZbBlkDesc*)bdesc, seqs, lits,
-                                                                                         dst, ptr, blk_first, blk_last, dict);
+                                                                                         dst, ptr, blk_first, blk_last, dict, chain);
     u64 const want = (hi - lo + 255) / 256;
     unsigned const grid = (unsigned)(want < n_ctas * 16ull ? want : n_ctas * 16ull);
     int rounds = 0;
@@ -1741,10 +1766,10 @@ static int zb_chase_run(const u8* src, const ZbFramePlace* place, const u32* sta
 
 int zb_launch_execute_chase(const u8* src, const ZbFramePlace* place, const u32* status, const ZbBlock* blocks, const void* bdesc,
                             const ZbSeq* seqs, const u8* lits, u8* dst, u64 lo, u64 hi, u64 n_total, u64 blk_first, u64 blk_last,
-                            void* ptr_mem, u32* d_changed, u32 n_ctas, ZbDictDev dict, cudaStream_t st)
+                            void* ptr_mem, u32* d_changed, u32 n_ctas, ZbDictDev dict, cudaStream_t st, int chain)
 {
-    if (n_total < (1ull << 31)) return zb_chase_run<u32>(src, place, status, blocks, bdesc, seqs, lits, dst, lo, hi, n_total, blk_first, blk_last, ptr_mem, d_changed, n_ctas, dict, st);
-    return zb_chase_run<u64>(src, place, status, blocks, bdesc, seqs, lits, dst, lo, hi, n_total, blk_first, blk_last, ptr_mem, d_changed, n_ctas, dict, st);
+    if (n_total < (1ull << 31)) return zb_chase_run<u32>(src, place, status, blocks, bdesc, seqs, lits, dst, lo, hi, n_total, blk_first, blk_last, ptr_mem, d_changed, n_ctas, dict, st, chain != 0);
+    return zb_chase_run<u64>(src, place, status, blocks, bdesc, seqs, lits, dst, lo, hi, n_total, blk_first, blk_last, ptr_mem, d_changed, n_ctas, dict, st, chain != 0);
 }
 
 size_t zb_wave_bytes(u64 n_frames, u64 n_blocks) { return (size_t)(n_frames * 12 + n_blocks * 4 + 64); }
@@ -1797,6 +1822,11 @@ void zb_launch_finish(const ZbFramePlace* place, const u64* out_sizes, const u32
                       u32* first_error, cudaStream_t st)
 {
     zb_finish<<<(n + 255) / 256, 256, 0, st>>>(place, out_sizes, status, n, out_segs, first_error);
+}
+
+void zb_launch_chain_shift(ZbFramePlace* place, u32 n, u64 carry, cudaStream_t st)
+{
+    zb_chain_shift<<<(n + 1 + 255) / 256, 256, 0, st>>>(place, n + 1, carry);
 }
 
 void zb_entropy_phase_read(unsigned long long* out8, int reset)

@@ -19,6 +19,8 @@
  *                               ranges balanced by bytes   c-ext/compressor.c:1127,1183-1200; c-ext/decompressor.c:1237,1290-1305
  *   zb200_dparams               ZstdDecompressor(max_window_size=) -> ZSTD_DCtx_setMaxWindowSize   c-ext/decompressor.c:17-60
  *   zb200_decompress_chain      ZstdDecompressor.decompress_content_dict_chain   c-ext/decompressor.c:620-890
+ *   zb200_compress_chain        the per-revision ZSTD_CCtx_refPrefix + ZSTD_compress2 loop that writes such a chain (no entry
+ *                               point of the reference; tests/chain_ref.py:compress_chain restates the loop)
  *   zb200_cparams.window_log    ZSTD_c_windowLog of ZstdCompressionParameters   c-ext/compressionparams.c:46
  *   zb200_host_copy             the write into the result PyBytes   c-ext/decompressor.c:283-352
  *   ZB200_SRC/DST_DEVICE, ZB200_SEGS_HOST, zb200_pointer_device: no counterpart (device-resident callers, SURVEY.md 8(f)-2)
@@ -174,6 +176,16 @@ int zb200_compress_batch_multi(const int* devices, int n_devices, const void* sr
 /* same, from an array of independent host buffers (list input, c-ext/compressor.c:1434-1466) */
 int zb200_compress_batch_ptrs(zb200_ctx* ctx, const void* const* srcs, const size_t* sizes, size_t n,
                               const zb200_cparams* params, const zb200_ddict* dict, uint32_t flags, zb200_result** out);
+/* ---- content-dictionary chains, compression: the inverse of zb200_decompress_chain.  srcs[k] (sizes[k] bytes, host memory) is
+ * revision k; *out holds n segments, frame k for chunk k.  Frame 0 is what zb200_compress_batch_ptrs writes for chunk 0 with
+ * `dict` and `params`, except that its content size is always written.  Every frame k >= 1 is chunk k compressed with chunk
+ * k-1 as a raw-content prefix: single segment (window = content size), content size, dictionary ID 0, a checksum when
+ * params->write_checksum is set; its match sources may lie anywhere in chunk k-1 (DESIGN.md section 4).  The chunks are cut into runs sized to free device
+ * memory (ZB200_CHAIN_RUN_BYTES overrides the budget, for tests); each run carries the previous run's last chunk as its
+ * prefix, and the frames do not depend on where the runs are cut.  A chunk of ZB_FAR_WINDOW (2 GiB - 128 MiB) bytes or more,
+ * or with its predecessor that many, fails the call: the chain decoder refuses such chunks. */
+int zb200_compress_chain(zb200_ctx* ctx, const void* const* srcs, const size_t* sizes, size_t n,
+                         const zb200_cparams* params, const zb200_ddict* dict, zb200_result** out);
 /* ZSTD_compressBound (zstd/zstd.c:4547) */
 uint64_t zb200_compress_bound(uint64_t src_size);
 
@@ -197,7 +209,7 @@ int zb200_train_dictionary(zb200_ctx* ctx, const void* samples, const size_t* si
                            void* out, size_t capacity, size_t* out_size, uint32_t* chosen_k, uint32_t* chosen_d);
 
 /* ---- result accessors */
-const void*          zb200_result_data(const zb200_result* r);       /* host (pinned) or device pointer */
+const void*          zb200_result_data(const zb200_result* r);       /* host (pinned; pageable for zb200_compress_chain) or device pointer */
 uint64_t             zb200_result_size(const zb200_result* r);       /* bytes in data */
 size_t               zb200_result_count(const zb200_result* r);
 const zb200_segment* zb200_result_segments(const zb200_result* r);   /* host array, count entries */
@@ -220,6 +232,7 @@ int zb200_frame_info(const void* src, size_t size, zb200_frame_info_t* out);
 #define ZB200_K_LAYOUT   6
 #define ZB200_K_FRAMES   7
 #define ZB200_K_VERIFY   8
+#define ZB200_K_CHAIN_INDEX 9   /* zb_chain_index (zb200_compress_chain) */
 #define ZB200_K_COUNT    16
 void zb200_profile_enable(zb200_ctx* ctx, int on);
 void zb200_profile_reset(zb200_ctx* ctx);

@@ -84,6 +84,7 @@ def lib():
             "zb200_decompress_chain": (i, [vp, vp, vp, sz, vp, vp, C.POINTER(vp)]),
             "zb200_compress_batch": (i, [vp, vp, vp, sz, vp, vp, u32, C.POINTER(vp)]),
             "zb200_compress_batch_ptrs": (i, [vp, vp, vp, sz, vp, vp, u32, C.POINTER(vp)]),
+            "zb200_compress_chain": (i, [vp, vp, vp, sz, vp, vp, C.POINTER(vp)]),
             "zb200_compress_bound": (u64, [u64]),
             "zb200_result_data": (vp, [vp]),
             "zb200_result_size": (u64, [vp]),

@@ -318,6 +318,57 @@ class ZstdCompressor:
         ctx.check(rc, "zb200_compress_batch")
         return res
 
+    # ------------------------------------------------------------------ content-dictionary chains
+    _FAR_WINDOW = (1 << 31) - (1 << 27)          # ZB_FAR_WINDOW (csrc/zb_common.cuh)
+
+    def compress_content_dict_chain(self, chunks):
+        """The inverse of ZstdDecompressor.decompress_content_dict_chain (not a method of the reference): frame k is chunks[k]
+        compressed with chunks[k - 1] as a raw-content prefix, so that the decompressor rebuilds chunks[k] from frames[:k + 1].
+
+        Frame 0 is what compress(chunks[0]) writes, with this compressor's dictionary, level, dictionary-ID flag and
+        parameters -- except that the chain format needs content sizes, so every frame carries one whatever
+        write_content_size says.  Frames 1.. are single-segment frames (the window is the content size) with no dictionary
+        ID and a checksum when write_checksum is set; their match sources may lie anywhere in the previous chunk, where the
+        reference's loop over ZSTD_CCtx_refPrefix reaches only its window.  The whole chain is one batch on the default
+        device.  A chunk of 2 GiB - 128 MiB or more, or with its predecessor that many bytes, raises ZstdError: the chain
+        decoder does not take it."""
+        if not isinstance(chunks, list):
+            raise TypeError("compress_content_dict_chain() argument 1 must be list, not %s" % type(chunks).__name__)
+        if not chunks:
+            raise ValueError("empty input chain")
+        views = []
+        for i, item in enumerate(chunks):
+            try:
+                v = memoryview(item)
+            except TypeError:
+                raise TypeError("item %d not a bytes like object" % i)
+            if not v.contiguous:
+                raise TypeError("item %d not a bytes like object" % i)
+            views.append(v)
+        for k, v in enumerate(views):
+            if v.nbytes >= self._FAR_WINDOW or (k and views[k - 1].nbytes + v.nbytes >= self._FAR_WINDOW):
+                raise ZstdError("chunk %d is too large for a content-dictionary chain: size, or previous plus own size, of "
+                                "2 GiB - 128 MiB or more" % k)
+        n = len(views)
+        arrs = [np.frombuffer(v, dtype=np.uint8) if v.nbytes else np.zeros(0, dtype=np.uint8) for v in views]
+        ctx = _native.Context.get(_native.default_device())
+        L = ctx.L
+        ptrs = (C.c_void_p * n)(*[a.ctypes.data if len(a) else None for a in arrs])
+        lens = (C.c_size_t * n)(*[len(a) for a in arrs])
+        p = self._params()
+        p.write_content_size = 1
+        dd = self._dict(ctx)
+        res = C.c_void_p()
+        with ctx.lock:
+            rc = L.zb200_compress_chain(ctx.h, ptrs, lens, n, C.byref(p), dd, C.byref(res))
+        ctx.check(rc, "zb200_compress_chain")
+        try:
+            base = L.zb200_result_data(res)
+            segs = (_native.Segment * n).from_address(L.zb200_result_segments(res))
+            return [_native.bytes_from_address(base + s.offset, s.length) for s in segs]
+        finally:
+            L.zb200_result_free(res)
+
     # ------------------------------------------------------------------ out of scope (SURVEY.md section 2, row 15)
     def _unsupported(self, *a, **k):
         raise NotImplementedError("streaming compression objects are outside the GPU batch path")

@@ -62,6 +62,11 @@ void zb_launch_compress_blocks(const u8* src, const void* jobs, u32 n_jobs, void
                                u32* stats = nullptr);
 u32 zb_encode_small_max();
 void zb_launch_dict_table(const u8* tail, u32 D, u16* table, cudaStream_t st);
+size_t zb_encode_pscratch_bytes();
+size_t zb_chain_seg_bytes();
+void zb_launch_chain_index(const u8* src, const void* segs, const u64* pos_off, u32 n_segs, u64 total_pos, u32 sms, cudaStream_t st);
+void zb_launch_compress_chain_blocks(const u8* src, const void* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes,
+                                     void* outs, u32* work_counter, const void* segs, cudaStream_t st);
 u32 zb_encode_ctable_bytes();
 void zb_launch_dict_ctables(const void* digest, void* out3, cudaStream_t st);
 void zb_launch_frame_layout(const ZbSegment* segs, const void* seginfo, const void* outs, u32 n_segs, u32 checksum, u32 content_size,
@@ -123,6 +128,7 @@ struct zb200_ctx {
     DevBuf biglist;                           // frames whose scans are a warp's work (zb_scan_frames_big)
     DevBuf chase;                             // its pointer-jumping execute stage: a source pointer per output byte
     DevBuf carry;                             // content-dictionary chains: the last fulltext of a run, the prefix of the next
+    DevBuf chain_tab, chain_seg, chain_pos;   // chain compression: the chunk indexes of a run, their descriptors, sampled positions
     int last_chase_rounds = 0;
     const char* last_compress_kernel = "";    // which of the three block kernels the last compress call ran (profile slot zb_compress_blocks)
     u32 entropy_warps = 0;
@@ -147,6 +153,7 @@ struct zb200_ddict {
 struct zb200_result {
     zb200_ctx* ctx; void* data = nullptr; bool data_on_device = false; bool data_pinned_pool = false;
     bool data_owned_device = false;        // ZB200_DST_DEVICE: the result owns its device allocation (stream-ordered pool)
+    std::vector<u8> host_data;             // zb200_compress_chain: the frames, in pageable memory the result owns
     u64 size = 0; size_t n = 0;
     std::vector<zb200_segment> segs;
     bool has_error = false; size_t err_item = 0; int err_code = 0; u64 err_got = 0, err_expected = 0;
@@ -251,6 +258,7 @@ void zb200_ctx_destroy(zb200_ctx* ctx)
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
     ctx->bdesc.release(); ctx->bexit.release(); ctx->erep.release(); ctx->fend.release(); ctx->wave.release(); ctx->chase.release(); ctx->biglist.release(); ctx->carry.release();
+    ctx->chain_tab.release(); ctx->chain_seg.release(); ctx->chain_pos.release();
     DevBuf* all[] = {&ctx->src, &ctx->segs, &ctx->dst_sizes, &ctx->info, &ctx->place, &ctx->status, &ctx->out_sizes,
                      &ctx->blocks, &ctx->seqs, &ctx->lits, &ctx->dst, &ctx->lane, &ctx->small, &ctx->out_segs, &ctx->partial,
                      &ctx->jobs, &ctx->seginfo, &ctx->slots, &ctx->bouts, &ctx->escratch, &ctx->fsizes, &ctx->ck};
@@ -971,6 +979,153 @@ int zb200_compress_batch_ptrs(zb200_ctx* ctx, const void* const* srcs, const siz
     return rc;
 }
 
+// ---------------------------------------------------------------- content-dictionary chains, compression
+// The inverse of zb200_decompress_chain: frame k is chunk k compressed with chunk k-1 as a raw-content prefix.  Chunk 0 goes
+// through the batch path with the dictionary; every later chunk is independent work once all chunks are known, so a run of
+// them is one batch: the chunks back to back on the device (chunk k-1 directly in front of chunk k), an index per chunk
+// (zb_chain_index), every block through the prefix mode of zb_compress_blocks, the frames laid out by the batch kernels with
+// window_log 31 (single segment: the window is the content size, so offsets may reach the whole prefix, RFC 8878 section 3.1.1.1.2).
+namespace {
+u32 chain_log(u64 len)          // a chunk's index: 2^log slots for the two keys of its sampled positions at a load of at most 1/2, >= 16 slots
+{
+    u64 const npos = len >= 8 ? (len - 8) / 4 + 1 : 0;
+    u32 L = 4; while ((1ull << L) < 4 * npos) L++;
+    return L;
+}
+struct HostChainSeg { u64 start; const u32* tab; const u32* prev_tab; u32 len, prev_len, log, prev_log; };    // == ZeChainSeg
+}
+
+int zb200_compress_chain(zb200_ctx* ctx, const void* const* srcs, const size_t* sizes, size_t n,
+                         const zb200_cparams* params, const zb200_ddict* dict, zb200_result** out)
+{
+    *out = nullptr;
+    if (!ctx || !srcs || !sizes || n == 0 || n > 0x7FFFFFF0u) return fail(ctx, "zb200_compress_chain: bad arguments", cudaSuccess);
+    if (sizeof(HostChainSeg) != zb_chain_seg_bytes()) return fail(ctx, "zb200_compress_chain: descriptor layout", cudaSuccess);
+    for (size_t k = 0; k < n; k++)       // the chain decoder's limit (ZB_FAR_WINDOW); the Python layer checks it first
+        if (sizes[k] >= ZB_FAR_WINDOW || (k && sizes[k - 1] + sizes[k] >= ZB_FAR_WINDOW)) return fail(ctx, "zb200_compress_chain: chunk of ZB_FAR_WINDOW or more", cudaSuccess);
+    cudaSetDevice(ctx->device);
+    zb200_cparams P; if (params) P = *params; else { memset(&P, 0, sizeof P); P.level = 3; }
+    P.write_content_size = 1;
+    std::vector<u8> host;                       // the frames, back to back (becomes the result's buffer)
+    std::vector<zb200_segment> fsegs(n);
+    // ---- chunk 0: the batch path, exactly as compress() with content size on
+    {
+        zb200_result* r0 = nullptr;
+        int rc = zb200_compress_batch_ptrs(ctx, srcs, sizes, 1, &P, dict, 0, &r0);
+        if (rc) return rc;
+        host.assign((const u8*)r0->data, (const u8*)r0->data + r0->size);
+        fsegs[0].offset = 0; fsegs[0].length = r0->size;
+        zb200_result_free(r0);
+    }
+    // ---- runs of chunks 1..n-1.  Device bytes per input byte: 1 (input) + <= 8 (index, two keys per 4 bytes) + ~1 (block slots); the budget is most
+    // of the free device memory, or ZB200_CHAIN_RUN_BYTES (read per call: tests force runs)
+    u64 budget;
+    {
+        const char* env = getenv("ZB200_CHAIN_RUN_BYTES");
+        size_t fr = 0, tot = 0; cudaMemGetInfo(&fr, &tot);
+        budget = env && *env ? strtoull(env, nullptr, 10) : (u64)fr / 10 * 6;
+    }
+    auto cost = [&](size_t j) { return (u64)sizes[j] + (4ull << chain_log(sizes[j])) + sizes[j] + (sizes[j] >> 7) + 4096 + 200 * (sizes[j] / ZB_BLOCK_MAX + 1); };
+    u64 const slot_bytes = ((u64)ZB_BLOCK_MAX + (ZB_BLOCK_MAX >> 7) + 64 + 15) & ~15ull;
+    u32 const ctas_max = (u32)ctx->sm_count * (227u * 1024u / zb_encode_smem_bytes());
+    size_t k = 1;
+    while (k < n) {
+        size_t b = k + 1; u64 use = cost(k - 1) + cost(k);
+        while (b < n && use + cost(b) <= budget) use += cost(b++);
+        size_t const m = b - (k - 1);            // staged chunks: k-1 (the prefix) .. b-1
+        // pinned staging: 64 bytes of slack on both sides (the kernels read a few bytes around what they compare)
+        u64 total = 0; for (size_t j = k - 1; j < b; j++) total += sizes[j];
+        u8* stage = (u8*)pinned_get(ctx, total + 128);
+        if (!stage) return fail(ctx, "pinned staging allocation", cudaErrorMemoryAllocation);
+        memset(stage, 0, 64); memset(stage + 64 + total, 0, 64);
+        std::vector<HostChainSeg> cs(m); std::vector<u64> tab_off(m + 1, 0), pos_off(m + 1, 0);
+        {
+            u64 pos = 64;
+            for (size_t i = 0; i < m; i++) {
+                size_t const j = k - 1 + i;
+                if (sizes[j]) memcpy(stage + pos, srcs[j], sizes[j]);
+                cs[i].start = pos; cs[i].len = (u32)sizes[j]; cs[i].log = chain_log(sizes[j]);
+                cs[i].prev_len = i ? (u32)sizes[j - 1] : 0; cs[i].prev_log = i ? cs[i - 1].log : 0;
+                tab_off[i + 1] = tab_off[i] + (1ull << cs[i].log);
+                pos_off[i + 1] = pos_off[i] + (sizes[j] >= 8 ? (sizes[j] - 8) / 4 + 1 : 0);
+                pos += sizes[j];
+            }
+        }
+        // block jobs of the chunks after the prefix; job.seg indexes the run's descriptors, the layout tables its frames
+        std::vector<HostJob> jobs; std::vector<HostSegInfo> sinfo(m - 1); std::vector<zb200_segment> lsegs(m - 1);
+        for (size_t i = 1; i < m; i++) {
+            u64 const len = cs[i].len;
+            lsegs[i - 1].offset = cs[i].start; lsegs[i - 1].length = len;
+            sinfo[i - 1].first_job = jobs.size(); sinfo[i - 1].n_jobs = 0; sinfo[i - 1].pad = 0;
+            for (u64 pos = 0; pos < len;) {
+                u32 const sz = (u32)(len - pos < ZB_BLOCK_MAX ? len - pos : ZB_BLOCK_MAX);
+                HostJob j; j.src_pos = cs[i].start + pos; j.size = sz; j.seg = (u32)i; j.first = pos == 0; j.last = pos + sz == len;
+                jobs.push_back(j); sinfo[i - 1].n_jobs++; pos += sz;
+            }
+        }
+        size_t const nj = jobs.size(), nf = m - 1;
+        u32 ctas = ctas_max; if (ctas > nj) ctas = (u32)nj; if (ctas == 0) ctas = 1;
+        cudaError_t e = ctx->src.ensure(total + 128);
+        if (e == cudaSuccess) e = ctx->chain_tab.ensure(tab_off[m] * 4);
+        if (e == cudaSuccess) e = ctx->chain_seg.ensure(m * sizeof(HostChainSeg));
+        if (e == cudaSuccess) e = ctx->chain_pos.ensure((m + 1) * sizeof(u64));
+        if (e == cudaSuccess) e = ctx->segs.ensure(nf * sizeof(ZbSegment));
+        if (e == cudaSuccess) e = ctx->jobs.ensure((nj + 1) * sizeof(HostJob));
+        if (e == cudaSuccess) e = ctx->seginfo.ensure(nf * sizeof(HostSegInfo));
+        if (e == cudaSuccess) e = ctx->slots.ensure((nj + 1) * slot_bytes);
+        if (e == cudaSuccess) e = ctx->bouts.ensure((nj + 1) * 8);
+        if (e == cudaSuccess) e = ctx->escratch.ensure((size_t)ctas * zb_encode_pscratch_bytes());
+        if (e == cudaSuccess) e = ctx->fsizes.ensure(nf * sizeof(u64));
+        if (e == cudaSuccess) e = ctx->out_segs.ensure(nf * sizeof(ZbSegment));
+        if (e == cudaSuccess) e = ctx->small.ensure(256);
+        if (e != cudaSuccess) { pinned_put(ctx, stage); return fail(ctx, "zb200_compress_chain allocation", e); }
+        u8* const d_src = ctx->src.as<u8>(); u32* const d_tab = ctx->chain_tab.as<u32>();
+        for (size_t i = 0; i < m; i++) { cs[i].tab = d_tab + tab_off[i]; cs[i].prev_tab = i ? d_tab + tab_off[i - 1] : nullptr; }
+        u64* d_total = ctx->small.as<u64>(); u32* d_counter = (u32*)(d_total + 8);
+        e = cudaMemcpyAsync(d_src, stage, total + 128, cudaMemcpyHostToDevice, ctx->stream);
+        if (e == cudaSuccess) e = cudaMemsetAsync(d_tab, 0xFF, tab_off[m] * 4, ctx->stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->chain_seg.p, cs.data(), m * sizeof(HostChainSeg), cudaMemcpyHostToDevice, ctx->stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->chain_pos.p, pos_off.data(), (m + 1) * sizeof(u64), cudaMemcpyHostToDevice, ctx->stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->segs.p, lsegs.data(), nf * sizeof(ZbSegment), cudaMemcpyHostToDevice, ctx->stream);
+        if (e == cudaSuccess && nj) e = cudaMemcpyAsync(ctx->jobs.p, jobs.data(), nj * sizeof(HostJob), cudaMemcpyHostToDevice, ctx->stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->seginfo.p, sinfo.data(), nf * sizeof(HostSegInfo), cudaMemcpyHostToDevice, ctx->stream);
+        if (e == cudaSuccess) e = cudaMemsetAsync(d_counter, 0, 64, ctx->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);          // (the staging block goes back to the pool)
+        pinned_put(ctx, stage);
+        if (e != cudaSuccess) return fail(ctx, "zb200_compress_chain upload", e);
+        { KSpan s(ctx, ZB200_K_CHAIN_INDEX);
+          zb_launch_chain_index(d_src, ctx->chain_seg.p, ctx->chain_pos.as<u64>(), (u32)m, pos_off[m], (u32)ctx->sm_count, ctx->stream); }
+        if (nj) { KSpan s(ctx, ZB200_K_COMPRESS);
+          zb_launch_compress_chain_blocks(d_src, ctx->jobs.p, (u32)nj, ctx->escratch.p, ctas, ctx->slots.as<u8>(), slot_bytes, ctx->bouts.p, d_counter,
+                                          ctx->chain_seg.p, ctx->stream); }
+        { KSpan s(ctx, ZB200_K_LAYOUT);
+          zb_launch_frame_layout(ctx->segs.as<ZbSegment>(), ctx->seginfo.p, ctx->bouts.p, (u32)nf, P.write_checksum ? 1 : 0, 1, 0, 31,
+                                 ctx->fsizes.as<u64>(), ctx->out_segs.as<ZbSegment>(), d_total, ctx->stream); }
+        u64 ftotal = 0;
+        CK(cudaMemcpyAsync(&ftotal, d_total, sizeof ftotal, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        CK(ctx->dst.ensure(ftotal + 64));
+        { KSpan s(ctx, ZB200_K_FRAMES);
+          zb_launch_write_frames(d_src, ctx->segs.as<ZbSegment>(), ctx->seginfo.p, ctx->bouts.p, ctx->slots.as<u8>(), slot_bytes, (u32)nf,
+                                 P.write_checksum ? 1 : 0, 1, 0, 31, ctx->out_segs.as<ZbSegment>(), ctx->dst.as<u8>(), ctx->stream); }
+        std::vector<ZbSegment> osegs(nf);
+        size_t const base = host.size();
+        host.resize(base + ftotal);
+        CK(cudaMemcpyAsync(osegs.data(), ctx->out_segs.p, nf * sizeof(ZbSegment), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaMemcpyAsync(host.data() + base, ctx->dst.p, ftotal, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        if (ctx->prof) fold_spans(ctx);
+        for (size_t f = 0; f < nf; f++) { fsegs[k + f].offset = base + osegs[f].offset; fsegs[k + f].length = osegs[f].length; }
+        k = b;
+    }
+    // ---- the result owns the buffer the runs were copied into (no second host copy)
+    zb200_result* res = new zb200_result();
+    res->ctx = ctx; res->n = n; res->size = host.size(); res->segs = fsegs;
+    res->host_data = std::move(host); res->data = res->host_data.data();
+    *out = res;
+    return 0;
+}
+
 uint64_t zb200_compress_bound(uint64_t n) { return n + (n >> 8) + (n < (128u << 10) ? (((128u << 10) - n) >> 11) : 0); }
 
 const void* zb200_result_data(const zb200_result* r) { return r->data; }
@@ -1029,7 +1184,8 @@ int zb200_profile_read(zb200_ctx* ctx, float ms[ZB200_K_COUNT], uint32_t launche
 const char* zb200_kernel_name(int k)
 {
     static const char* names[ZB200_K_COUNT] = {"zb_scan_frames", "zb_place_frames", "zb_entropy_decode", "zb_execute", "zb_finish",
-                                                "zb_compress_blocks", "zb_frame_layout", "zb_write_frames", "zb_verify_checksums"};
+                                                "zb_compress_blocks", "zb_frame_layout", "zb_write_frames", "zb_verify_checksums",
+                                                "zb_chain_index"};
     return (k >= 0 && k < ZB200_K_COUNT && names[k]) ? names[k] : "";
 }
 // ---------------------------------------------------------------- one batch over several devices

@@ -88,6 +88,38 @@ struct ZeScratch {
     u32 tmp_seq[(ZE_BLOCK + 1024) / 4]; // sequence bitstream
     u16 distL[ZE_BLOCK + 64];           // dual-table mode: distance to the nearest earlier position with the same 8-byte hash
 };
+// Prefix mode (content-dictionary chains) needs 32-bit distances and match lengths beyond the 12 bits of the compacted
+// record, and a sequence bitstream beyond tmp_seq (30-bit offsets on 4-byte matches); the other modes keep their scratch as
+// it is.
+#define ZE_PSEQ_BITS 88u                // most bits of one sequence: states 9 + 8 + 9, LL 16, ML 16, OF 30
+struct ZePScratch : ZeScratch {
+    u32 dist32[ZE_BLOCK + 64];          // distance of the verified index candidate of every position, 0 = none
+    u32 seqml[ZE_MAXSEQ + 8];           // match length of compacted sequence i (seq[i] = {ll, offBase})
+    u32 seqbits[(ZE_MAXSEQ * ZE_PSEQ_BITS + 32 * 4) / 32 + 4];   // the sequence bitstream (tmp_seq's job in the other modes)
+};
+static_assert(sizeof(ZePScratch::seqbits) * 8 >= (size_t)ZE_MAXSEQ * ZE_PSEQ_BITS + 26 + 1 + 2 * 32 + 64,
+              "the prefix-mode bitstream must hold the worst block: every sequence at its widest, the final states, the zeroed tail");
+// one chunk of a chain run as the prefix-mode kernel sees it: its bytes, its index, and those of the chunk in front of it
+// (which lies directly in front of it in the run's buffer)
+struct ZeChainSeg {
+    u64 start;                          // byte position of the chunk in src
+    const u32* tab;                     // its index: 2^log u32 slots, the earliest sampled position of every key (two per position)
+    const u32* prev_tab;                // the previous chunk's index (nullptr: none)
+    u32 len, prev_len, log, prev_log;
+};
+#define ZE_CHAIN_STEP 4u                // the index samples every 4th position; backward extension finds the true starts
+// An index slot is keyed on the 8 bytes at a position AND on the position's 4 KiB bucket: in a revision the bytes of
+// position p mostly sit near p in the previous revision, and a lookup probes the buckets around p.  Keyed on the bytes
+// alone, the earliest occurrence of a common 8-byte string (indentation, a keyword) would answer for all of them.
+#define ZE_CHAIN_BUCKET 12u
+__device__ __forceinline__ u32 ze_chain_slot(u64 v, u32 pos, u32 log)
+{
+    return (u32)(((v ^ ((u64)(pos >> ZE_CHAIN_BUCKET) * 0xC2B2AE3D27D4EB4Full)) * 0x9E3779B185EBCA87ull) >> (64 - log));
+}
+// The same table also keys every sampled position on the 32 bytes at it, whatever the position: this key finds a source
+// anywhere in the chunk (content moved, inserted or deleted by any amount).  32 bytes rather than 8, so that the earliest
+// occurrence of the key is rarely a repeat of the bytes rather than their source.
+#define ZE_CHAIN_FAR 32u
 
 // ---------------------------------------------------------------------------
 // small helpers
@@ -126,6 +158,13 @@ __device__ __forceinline__ u32 ze_count(const u8* a, const u8* b, u32 limit)
     return m;
 }
 __device__ __forceinline__ u32 ze_hibit(u32 v) { return 31 - __clz(v); }
+// the chain index's position-free key (ZE_CHAIN_FAR bytes at p)
+__device__ __forceinline__ u32 ze_chain_far_slot(const u8* p, u32 log)
+{
+    u64 const h = ((((ze_ld64(p) * 0x9E3779B185EBCA87ull) ^ ze_ld64(p + 8)) * 0xC2B2AE3D27D4EB4Full ^ ze_ld64(p + 16)) * 0x165667B19E3779F9ull
+                   ^ ze_ld64(p + 24)) * 0x27D4EB2F165667C5ull;
+    return (u32)(h >> (64 - log));
+}
 
 __device__ __forceinline__ u32 ze_ll_code(u32 ll)       // ZSTD_LLcode, zstd/zstd.c:19738
 {
@@ -526,6 +565,15 @@ __device__ __forceinline__ u32 ze_off_code(u32 off, u32 ll, u32& r0, u32& r1, u3
     return ob;
 }
 
+// what a unit record keeps of a match's offset: its offBase, or in prefix mode the raw offset (phase D codes it per block);
+// the unit's repcode history is updated either way
+template <bool PREFIX>
+__device__ __forceinline__ u32 ze_rec_off(u32 off, u32 ll, u32& r0, u32& r1, u32& r2)
+{
+    u32 const ob = ze_off_code(off, ll, r0, r1, r2);
+    return PREFIX ? off : ob;
+}
+
 // DUAL = the reference's double-fast idea (zstd/zstd.c:31039) in the same 32 KB of shared memory: 2^13 heads keyed on 4
 // bytes plus 2^13 heads keyed on 8 bytes; a position takes its 8-byte candidate when that one verifies 8 bytes.  CPU
 // model tools/enc_model3.c: 128 KiB text +3.2 % -> -1.6 % against level 3.  Used for level >= 4; the default
@@ -533,7 +581,12 @@ __device__ __forceinline__ u32 ze_off_code(u32 off, u32 ll, u32& r0, u32& r1, u3
 // STATS (dictionary training only): every block coded as a compressed block adds its literal bytes and its LL / ML / OF code
 // histograms to stats[0..256), [256..292), [292..345), [345..377) -- the counts ZDICT_countEStats (zstd/zstd.c:53124) takes.
 // The pointer is null and unused in the other instantiations.
-template <bool DUAL, u32 UNIT, bool STATS = false>
+// PREFIX (content-dictionary chains, DUAL false, UNIT 1 KiB): a block's history is contiguous in front of `in` -- its own chunk
+// so far, then the whole previous chunk -- and dict.cct points to the run's ZeChainSeg table (job.seg indexes it).  Phase A
+// is a lookup of every position's 8-byte hash in the two chunk indexes (zb_chain_index) instead of the hash links; the
+// parse runs as in the other modes on 32-bit distances; the compaction merges matches that continue across unit borders
+// and re-derives the repcodes of the whole block; scratch is a ZePScratch array.
+template <bool DUAL, u32 UNIT, bool STATS = false, bool PREFIX = false>
 __global__ void __launch_bounds__(ZE_THREADS)
 zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jobs, u32 n_jobs,
                    ZeScratch* __restrict__ scratch, u8* __restrict__ slots, u64 slot_bytes,
@@ -541,7 +594,8 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
 {
     extern __shared__ __align__(16) u8 ze_smem_raw[];
     ZeShared& S = *(ZeShared*)ze_smem_raw;
-    ZeScratch& G = scratch[blockIdx.x];
+    ZeScratch& G = PREFIX ? (ZeScratch&)((ZePScratch*)scratch)[blockIdx.x] : scratch[blockIdx.x];
+    ZePScratch& GP = (ZePScratch&)G;            // (PREFIX only)
     u32 const tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     __shared__ u32 s_job;
 
@@ -575,9 +629,12 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
         // right in front of `in`); otherwise blocks are compressed independently
         constexpr u32 ZE_HIST = 32768;
         bool const hist = DUAL && !job.first;
-        u32 const D = job.first ? dict.D : (hist ? ZE_HIST : 0u);
-        const u8* const dict_end = hist ? in : dict.tail + dict.D;
-        bool const dict_first = DUAL ? job.first != 0 : true;       // dictionary entropy tables / repcodes belong to first blocks only
+        ZeChainSeg cs = {}; if constexpr (PREFIX) cs = ((const ZeChainSeg*)dict.cct)[job.seg];
+        u32 const bpos = PREFIX ? (u32)(job.src_pos - cs.start) : 0u;             // (PREFIX) block position in its chunk
+        // PREFIX: everything in front of the block back to the start of the previous chunk is history
+        u32 const D = PREFIX ? bpos + cs.prev_len : (job.first ? dict.D : (hist ? ZE_HIST : 0u));
+        const u8* const dict_end = (PREFIX || hist) ? in : dict.tail + dict.D;
+        bool const dict_first = PREFIX ? false : (DUAL ? job.first != 0 : true);  // dictionary entropy tables / repcodes belong to first blocks only
         bool const skip0 = job.first && D == 0;                    // without a dictionary the reference never uses position 0 as a match source
         u32 const n = job.size;
         constexpr u32 unit = UNIT;                                 // bytes each parse lane owns
@@ -608,12 +665,56 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
 
         ZE_MARK(0);
         // ---------------- A: hash links (warp 0); the other warps clear the histograms meanwhile
+        if constexpr (!PREFIX) {
         if (D && !hist) { const u32* t32 = (const u32*)dict.table; for (u32 i = tid; i < (1u << ZE_HLOG) / 2; i += ZE_THREADS) ((u32*)S.head)[i] = t32[i]; }
         else for (u32 i = tid; i < (1u << ZE_HLOG) / 2; i += ZE_THREADS) ((u32*)S.head)[i] = 0xFFFFFFFFu;
+        }
         for (u32 i = tid; i < 256; i += ZE_THREADS) S.hist[i] = 0;
         if (tid < 36) S.hLL[tid] = 0; if (tid < 32) S.hOF[tid] = 0; if (tid < 56) S.hML[tid] = 0;
         __syncthreads();
-        if (warp == 0) {
+        if constexpr (PREFIX) {
+            // every position (a thread each) looks its 8 bytes up in the previous chunk's index (the buckets around its own
+            // position) and in its own chunk's (its bucket and the one before, only candidates in front of it), and its 32
+            // bytes in both indexes without a bucket, which finds sources anywhere in the two chunks; every
+            // candidate is verified against the input (up to 32 bytes) and the best becomes the position's distance.  No
+            // shared table, so no races: the result does not depend on timing.
+            for (u32 p = tid; p < n; p += ZE_THREADS) {
+                u32 d = 0, dl = 0;
+                if (p + 8 <= n) {
+                    u64 const v = ze_ld64(in + p);
+                    u32 const cp = bpos + p, bk = cp >> ZE_CHAIN_BUCKET;
+                    u32 best = 0, best_len = 7, best_gap = 0xFFFFFFFFu;
+                    // candidate at chunk position q (dd bytes back): the longer verified match wins; on a tie the one nearer
+                    // to where the position's bytes sat in the previous chunk (gap), then the nearer one
+                    auto take = [&](u32 dd, u32 gap) {
+                        u32 const m = ze_count(in + p, in + p - dd, 32);
+                        if (m > best_len || (m == best_len && best && (gap < best_gap || (gap == best_gap && dd < best)))) { best = dd; best_len = m; best_gap = gap; }
+                    };
+                    if (cs.prev_tab) {
+                        for (u32 b = bk ? bk - 1 : 0; b <= bk + 1; b++) {
+                            u32 const q = cs.prev_tab[ze_chain_slot(v, b << ZE_CHAIN_BUCKET, cs.prev_log)];
+                            if (q != 0xFFFFFFFFu && q < cs.prev_len && (q >> ZE_CHAIN_BUCKET) == b) take(cp + cs.prev_len - q, q > cp ? q - cp : cp - q);
+                        }
+                    }
+                    for (u32 b = bk ? bk - 1 : 0; b <= bk; b++) {
+                        u32 const q = cs.tab[ze_chain_slot(v, b << ZE_CHAIN_BUCKET, cs.log)];
+                        if (q < cp && (q >> ZE_CHAIN_BUCKET) == b) take(cp - q, 0xFFFFFFFEu);
+                    }
+                    if (cp + ZE_CHAIN_FAR <= cs.len) {                 // anywhere in either chunk
+                        if (cs.prev_tab) {
+                            u32 const q = cs.prev_tab[ze_chain_far_slot(in + p, cs.prev_log)];
+                            if (q < cs.prev_len) take(cp + cs.prev_len - q, q > cp ? q - cp : cp - q);
+                        }
+                        u32 const q = cs.tab[ze_chain_far_slot(in + p, cs.log)];
+                        if (q < cp) take(cp - q, 0xFFFFFFFEu);
+                    }
+                    d = best; dl = best ? best_len : 0u;
+                }
+                GP.dist32[p] = d; G.distL[p] = (u16)dl;        // (distL: the verified length, for the units' hints below)
+            }
+            __syncthreads();
+        }
+        if (!PREFIX && warp == 0) {
             u32 const lt = (1u << lane) - 1;
             volatile u16* const vhead = S.head;      // one warp, converged every step: table accesses stay in program order
             bool const exact = n < 2048;
@@ -768,6 +869,7 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
         // entry) and then decides, so a step costs one memory round trip for the whole warp instead of
         // one per divergent path.  Long matches continue in EXTEND iterations, 8 bytes per step.
         {
+            auto dist_at = [&](u32 i) -> u32 { if constexpr (PREFIX) return GP.dist32[i]; else return G.dist[i]; };
             u32 const u0 = tid * unit;
             u32 cnt = 0, tail = 0;
             bool alive = u0 < n;
@@ -776,10 +878,36 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
             u32 ip = u0, anchor = u0, r0 = 0, r1 = 0, r2 = 0;
             if (alive && ip == 0 && skip0) ip = 1;                 // the reference starts its search at position 1 (zstd/zstd.c:31075)
             if (tid == 0 && dict_first && D && dict.ent) { r0 = dict.ent->rep[0]; r1 = dict.ent->rep[1]; r2 = dict.ent->rep[2]; }   // a frame with a dictionary starts from its repcodes (ZSTD_loadCEntropy)
+            if constexpr (PREFIX) {
+                // A unit starts with a guess of the offset the match that ran to the end of the unit before it had, as both
+                // repcodes: in a revision that match usually runs on, the repcode check at the unit's first byte picks it up,
+                // and D merges the two halves.  The guess: of the distance to the unit's own place in the previous chunk and
+                // the last 16 distinct candidates (verified >= 16 bytes) in front of the unit, the one whose match reaches
+                // furthest back from the unit's first byte (on a tie, further ahead).  Records keep raw offsets and D codes
+                // them against the true history, so these seeds never reach the output.
+                if (alive && u0 + D > 0) {
+                    u32 back = 0, guess = 0;
+                    auto try_guess = [&](u32 d) {
+                        u32 const lim = min(256u, u0 + D - d);
+                        const u8* const a = in + u0;
+                        u32 k = 0; while (k < lim && a[-1 - (int)k] == a[-1 - (int)k - (int)d]) k++;
+                        if (k == lim) k += ze_count(a, a - d, min(256u, n - u0));      // (a tie behind the unit: the longer run ahead)
+                        if (k > back) { back = k; guess = d; }
+                    };
+                    if (cs.prev_len) try_guess(cs.prev_len);                    // the unit's own place in the previous chunk
+                    u32 const lo = u0 > 256 ? u0 - 256 : 0; u32 seen = 0;
+                    for (u32 p = u0; p-- > lo && seen < 16;) {
+                        u32 const d = G.distL[p] >= 16 ? dist_at(p) : 0u;
+                        if (!d || d == guess || d > u0 + D) continue;
+                        seen++; try_guess(d);
+                    }
+                    if (guess) r0 = r1 = guess;
+                }
+            }
             uint2* const rec = G.useq + tid * ZE_UNIT_SEQ;
             u32 mode = 0, m_start = 0, m_off = 0, m_len = 0;
             u32 d0 = 0, d1 = 0;
-            if (alive) { d0 = G.dist[ip]; d1 = ip + 1 < n ? G.dist[ip + 1] : 0; }
+            if (alive) { d0 = dist_at(ip); d1 = ip + 1 < n ? dist_at(ip + 1) : 0; }
             for (;;) {
                 if (alive && mode == 1 && m_start + m_len + 8 > n) {        // the last bytes of a block: finish the match bytewise (no wide reads past the input)
                     while (m_start + m_len < end) {
@@ -789,9 +917,9 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
                         m_len++;
                     }
                     u32 const ll = m_start - anchor;
-                    rec[cnt++] = make_uint2(ll | (m_len << 16), ze_off_code(m_off, ll, r0, r1, r2));
+                    rec[cnt++] = make_uint2(ll | (m_len << 16), ze_rec_off<PREFIX>(m_off, ll, r0, r1, r2));
                     ip = m_start + m_len; anchor = ip; mode = 0;
-                    d0 = ip < n ? G.dist[ip] : 0; d1 = ip + 1 < n ? G.dist[ip + 1] : 0;
+                    d0 = ip < n ? dist_at(ip) : 0; d1 = ip + 1 < n ? dist_at(ip + 1) : 0;
                 }
                 bool const searching = alive && mode == 0 && ip + 4 <= end && ip < ilimit;   // ... and stops one short of ilimit (:31100-31180)
                 bool const extending = alive && mode == 1;
@@ -815,13 +943,15 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
                     has_rq = searching && anchor == ip && r1 != 0 && (int)ip - (int)r1 >= -(int)D;
                     // EXTEND has no use for the candidate slots, so they fetch the next 16 bytes of both sides (24 bytes per step).
                     // A further window counts only if it lies wholly inside the block and wholly on one side of the dictionary end.
-                    ext1 = extending && pa + 16 <= n && (pbi >= 0 || pbi + 16 <= 0);
-                    ext2 = ext1 && pa + 24 <= n && (pbi >= 0 || pbi + 24 <= 0);
+                    // (PREFIX: the history is contiguous with the block, so no window has to stay on one side of its start)
+                    ext1 = extending && pa + 16 <= n && (PREFIX || pbi >= 0 || pbi + 16 <= 0);
+                    ext2 = ext1 && pa + 24 <= n && (PREFIX || pbi >= 0 || pbi + 24 <= 0);
                     int const pci = has_c1 ? (int)ip + 1 - (int)d1 : (ext1 ? (int)pa + 8 : (int)pa);
                     int const ppi = has_rp ? (int)ip + 1 - (int)r0 : (ext1 ? pbi + 8 : (int)pa);
                     int const pqi = has_rq ? (int)ip - (int)r1 : (ext2 ? (int)pa + 16 : (int)pa);
                     int const pxi = ext2 ? pbi + 16 : (int)pa;
-                    capB = pbi < 0 ? (u32)(-pbi) : 64u; capC = pci < 0 ? (u32)(-pci) : 64u; capP = ppi < 0 ? (u32)(-ppi) : 64u; capQ = pqi < 0 ? (u32)(-pqi) : 64u;
+                    capB = !PREFIX && pbi < 0 ? (u32)(-pbi) : 64u; capC = !PREFIX && pci < 0 ? (u32)(-pci) : 64u;
+                    capP = !PREFIX && ppi < 0 ? (u32)(-ppi) : 64u; capQ = !PREFIX && pqi < 0 ? (u32)(-pqi) : 64u;
                     u32 const back_room = pbi >= 0 ? (u32)pbi : D - (u32)(-pbi);          // bytes available before the candidate
                     u32 const em = (searching && d0) ? min(4u, min(ip - anchor, back_room)) : 0u;   // bytes that may extend the match backwards
                     has_bk = em != 0; bk_max = em;
@@ -859,7 +989,7 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
                     const u32* const wka = ZE_W(qa) - 1; const u32* const wkb = ZE_W(qb) - 1;
                     u32 const ka = (has_bk && (uintptr_t)wka >= in_lo) ? *wka : 0u;
                     u32 const kb = (has_bk && (pbi < 0 || (uintptr_t)wkb >= in_lo)) ? *wkb : 0u;
-                    u32 const dn = (searching && ip + 2 < n) ? G.dist[ip + 2] : 0;
+                    u32 const dn = (searching && ip + 2 < n) ? dist_at(ip + 2) : 0;
                     #define ZE_J(x0, x1, x2, q) ((u64)__funnelshift_r(x0, x1, ZE_S(q)) | ((u64)__funnelshift_r(x1, x2, ZE_S(q)) << 32))
                     A = ZE_J(a0, a1, a2, qa); B = ZE_J(b0, b1, b2, qb); C1 = ZE_J(c0, c1, c2, qc); RP = ZE_J(p0, p1, p2, qp); RQ = ZE_J(q0, q1, q2, qq);
                     X2 = ZE_J(x0, x1, x2, qx);
@@ -901,7 +1031,7 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
                         u32 const step = 1 + ((ip - anchor) >> 8);
                         ip += step;
                         if (step == 1) { d0 = d1; d1 = d2; }
-                        else { d0 = ip < n ? G.dist[ip] : 0; d1 = ip + 1 < n ? G.dist[ip + 1] : 0; }
+                        else { d0 = ip < n ? dist_at(ip) : 0; d1 = ip + 1 < n ? dist_at(ip + 1) : 0; }
                     }
                 } else if (extending) {
                     u32 const room = end - (m_start + m_len);
@@ -913,9 +1043,9 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
                 }
                 if (fin) {
                     u32 const ll = f_start - anchor;
-                    rec[cnt++] = make_uint2(ll | (f_len << 16), ze_off_code(f_off, ll, r0, r1, r2));
+                    rec[cnt++] = make_uint2(ll | (f_len << 16), ze_rec_off<PREFIX>(f_off, ll, r0, r1, r2));
                     ip = f_start + f_len; anchor = ip; mode = 0;
-                    d0 = ip < n ? G.dist[ip] : 0; d1 = ip + 1 < n ? G.dist[ip + 1] : 0;
+                    d0 = ip < n ? dist_at(ip) : 0; d1 = ip + 1 < n ? dist_at(ip + 1) : 0;
                 }
             }
             if (u0 < n) tail = end - anchor;
@@ -925,6 +1055,31 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
 
         ZE_MARK(2);
         // ---------------- D: compaction of the units' sequences + literal gather
+        u32 nseq;
+        if constexpr (PREFIX) {
+            // One serial pass: a unit's leading match that continues the previous unit's trailing match (same offset, no
+            // literals between) is merged into it -- a revision that is one long match stays one sequence, not one per
+            // 1 KiB unit -- and every offset is coded against the block's own repcode history.  Repcodes start as zeros,
+            // which match no offset, so every repcode this emits names a slot the decoder holds the same value in.
+            if (tid == 0) {
+                u32 o = 0, carry = 0, last_off = 0, r0 = 0, r1 = 0, r2 = 0; u32 const units = (n + unit - 1) / unit;
+                for (u32 u = 0; u < units; u++) {
+                    const uint2* const rec = G.useq + u * ZE_UNIT_SEQ;
+                    u32 const c = S.ucnt[u];
+                    for (u32 k = 0; k < c; k++) {
+                        uint2 const r = rec[k];
+                        u32 const ll = (r.x & 0xFFFFu) + (k == 0 ? carry : 0u), ml = r.x >> 16, off = r.y;
+                        if (o && ll == 0 && off == last_off) { GP.seqml[o - 1] += ml; continue; }
+                        G.seq[o] = make_uint2(ll, off); GP.seqml[o] = ml; o++; last_off = off;
+                    }
+                    if (c) carry = S.utail[u]; else carry += S.utail[u];
+                }
+                for (u32 i = 0; i < o; i++) G.seq[i].y = ze_off_code(G.seq[i].y, G.seq[i].x, r0, r1, r2);
+                S.nseq = o; S.tail_lit = carry;
+            }
+            __syncthreads();
+            nseq = S.nseq;
+        } else {
         if (tid == 0) {
             u32 off = 0, carry = 0; u32 const units = (n + unit - 1) / unit;
             for (u32 u = 0; u < 128; u++) {
@@ -934,7 +1089,7 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
             S.nseq = off; S.tail_lit = carry;
         }
         __syncthreads();
-        u32 const nseq = S.nseq;
+        nseq = S.nseq;
         {
             u32 const c = S.ucnt[tid], o = S.uoff[tid];
             const uint2* const rec = G.useq + tid * ZE_UNIT_SEQ;
@@ -946,13 +1101,14 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
             }
         }
         __syncthreads();
+        }
         // codes, histograms, literal positions; gather literals
         {
             u32 lit_run = 0, src_run = 0;      // running prefix over chunks of 128 sequences
             for (u32 base = 0; base < nseq; base += ZE_THREADS) {
                 u32 const i = base + tid; bool const v = i < nseq;
                 uint2 const r = v ? G.seq[i] : make_uint2(0, 0);
-                u32 const ll = r.x, ml = r.y >> 20, ob = r.y & 0xFFFFFu;
+                u32 const ll = r.x, ml = PREFIX ? (v ? GP.seqml[i] : 0u) : r.y >> 20, ob = PREFIX ? r.y : r.y & 0xFFFFFu;
                 u32 tot_l, tot_s;
                 u32 const lpos = ze_block_scan(ll, S.s_warp, tot_l) + lit_run;
                 u32 const spos = ze_block_scan(ll + ml, S.s_warp, tot_s) + src_run;
@@ -1064,7 +1220,8 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
         }
 
         ZE_MARK(5);
-        // ---------------- E: sequences -> tmp_seq
+        // ---------------- E: sequences -> tmp_seq (PREFIX: seqbits)
+        u32* const tseq = PREFIX ? GP.seqbits : G.tmp_seq;
         u32 seq_payload = 0;
         if (nseq) {
             // three state chains, last sequence to first (warps 0..2, lane 0)
@@ -1121,27 +1278,27 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
             }
             u32 const total_bits = run + logML + logOF + logLL;
             seq_payload = (total_bits + 1 + 7) / 8;
-            for (u32 i = tid; i < seq_payload / 4 + 2; i += ZE_THREADS) G.tmp_seq[i] = 0;
+            for (u32 i = tid; i < seq_payload / 4 + 2; i += ZE_THREADS) tseq[i] = 0;
             __syncthreads();
             for (u32 i = tid; i < nseq; i += ZE_THREADS) {
                 uint2 const r = G.seq[i];
-                u32 const ll = r.x, ml = (r.y >> 20) - 3, ob = r.y & 0xFFFFFu;
+                u32 const ll = r.x, ml = (PREFIX ? GP.seqml[i] : r.y >> 20) - 3, ob = PREFIX ? r.y : r.y & 0xFFFFFu;
                 u32 bp = G.bitpos[i];
                 u32 const so = G.sbits[1][i], sm = G.sbits[2][i], sl = G.sbits[0][i];
-                ze_put_bits(G.tmp_seq, bp, so & 0xFFF, so >> 12); bp += so >> 12;     // OF, ML, LL state bits
-                ze_put_bits(G.tmp_seq, bp, sm & 0xFFF, sm >> 12); bp += sm >> 12;
-                ze_put_bits(G.tmp_seq, bp, sl & 0xFFF, sl >> 12); bp += sl >> 12;
+                ze_put_bits(tseq, bp, so & 0xFFF, so >> 12); bp += so >> 12;     // OF, ML, LL state bits
+                ze_put_bits(tseq, bp, sm & 0xFFF, sm >> 12); bp += sm >> 12;
+                ze_put_bits(tseq, bp, sl & 0xFFF, sl >> 12); bp += sl >> 12;
                 u32 const lb = e_LL_bits[G.llc[i]], mb = e_ML_bits[G.mlc[i]], obits = G.ofc[i];
-                ze_put_bits(G.tmp_seq, bp, ll, lb); bp += lb;                          // LL, ML, OF additional bits
-                ze_put_bits(G.tmp_seq, bp, ml, mb); bp += mb;
-                ze_put_bits(G.tmp_seq, bp, ob, obits);
+                ze_put_bits(tseq, bp, ll, lb); bp += lb;                          // LL, ML, OF additional bits
+                ze_put_bits(tseq, bp, ml, mb); bp += mb;
+                ze_put_bits(tseq, bp, ob, obits);
             }
             if (tid == 0) {
                 u32 bp = run;
-                ze_put_bits(G.tmp_seq, bp, G.sbits[2][nseq], logML); bp += logML;      // flush ML, OF, LL states
-                ze_put_bits(G.tmp_seq, bp, G.sbits[1][nseq], logOF); bp += logOF;
-                ze_put_bits(G.tmp_seq, bp, G.sbits[0][nseq], logLL); bp += logLL;
-                ze_put_bits(G.tmp_seq, bp, 1, 1);
+                ze_put_bits(tseq, bp, G.sbits[2][nseq], logML); bp += logML;      // flush ML, OF, LL states
+                ze_put_bits(tseq, bp, G.sbits[1][nseq], logOF); bp += logOF;
+                ze_put_bits(tseq, bp, G.sbits[0][nseq], logLL); bp += logLL;
+                ze_put_bits(tseq, bp, 1, 1);
             }
             __syncthreads();
         }
@@ -1206,7 +1363,7 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
                 else if (S.lit_mode == 0) { for (u32 i = tid; i < nlit; i += ZE_THREADS) o[p + i] = G.lit[i]; p += nlit; }
                 for (u32 i = tid; i < S.seq_hdr_bytes; i += ZE_THREADS) o[p + i] = S.seq_hdr_buf[i];
                 p += S.seq_hdr_bytes;
-                if (nseq) { const u8* ps = (const u8*)G.tmp_seq; for (u32 i = tid; i < seq_payload; i += ZE_THREADS) o[p + i] = ps[i]; }
+                if (nseq) { const u8* ps = (const u8*)tseq; for (u32 i = tid; i < seq_payload; i += ZE_THREADS) o[p + i] = ps[i]; }
             }
         }
         ZE_MARK(8);
@@ -1252,6 +1409,27 @@ __global__ void zb_dict_table(const u8* __restrict__ tail, u32 D, u16* __restric
         u32 const m = __match_any_sync(0xFFFFFFFFu, valid ? h : (0x10000u + lane));
         if (valid && (m >> lane) == 1u && (p & 0xFFFFu) != 0xFFFFu) table[h] = (u16)p;
         __syncwarp();
+    }
+}
+
+// ===========================================================================
+// content-dictionary chains: one index per chunk of a run (a thread per sampled position, grid-stride).  Position p of chunk
+// s (every ZE_CHAIN_STEP-th position with 8 bytes behind it) goes to slot ze_chain_slot(8 bytes, p) of the chunk's table, and
+// with ZE_CHAIN_FAR bytes behind it also to slot ze_chain_far_slot, by
+// atomicMin: the earliest position wins whatever the order the threads run in, so the table -- and with it every frame --
+// is the same on every run and on the CPU build.  pos_off[s] = sampled positions of the chunks before s (host prefix sum).
+// ===========================================================================
+__global__ void __launch_bounds__(256)
+zb_chain_index(const u8* __restrict__ src, const ZeChainSeg* __restrict__ segs, const u64* __restrict__ pos_off, u32 n_segs)
+{
+    u64 const total = pos_off[n_segs];
+    for (u64 g = (u64)blockIdx.x * blockDim.x + threadIdx.x; g < total; g += (u64)gridDim.x * blockDim.x) {
+        u32 lo = 0, hi = n_segs;                     // the chunk: last s with pos_off[s] <= g
+        while (hi - lo > 1) { u32 const mid = (lo + hi) >> 1; if (pos_off[mid] <= g) lo = mid; else hi = mid; }
+        ZeChainSeg const& c = segs[lo];
+        u32 const p = (u32)(g - pos_off[lo]) * ZE_CHAIN_STEP;
+        atomicMin((u32*)&c.tab[ze_chain_slot(ze_ld64(src + c.start + p), p, c.log)], p);
+        if (p + ZE_CHAIN_FAR <= c.len) atomicMin((u32*)&c.tab[ze_chain_far_slot(src + c.start + p, c.log)], p);
     }
 }
 
@@ -1412,6 +1590,25 @@ void zb_launch_compress_blocks(const u8* src, const void* jobs, u32 n_jobs, void
     else if (dual) { if (small_blocks) ZE_LAUNCH(true, ZE_UNIT_SMALL, false); else ZE_LAUNCH(true, ZE_UNIT, false); }
     else           { if (small_blocks) ZE_LAUNCH(false, ZE_UNIT_SMALL, false); else ZE_LAUNCH(false, ZE_UNIT, false); }
     #undef ZE_LAUNCH
+}
+
+// content-dictionary chains: the chunk indexes of a run, and its block jobs through the prefix mode
+size_t zb_encode_pscratch_bytes() { return sizeof(ZePScratch); }
+size_t zb_chain_seg_bytes() { return sizeof(ZeChainSeg); }
+void zb_launch_chain_index(const u8* src, const void* segs, const u64* pos_off, u32 n_segs, u64 total_pos, u32 sms, cudaStream_t st)
+{
+    if (!total_pos) return;
+    u64 const want = (total_pos + 255) / 256; u32 const grid = (u32)(want < (u64)sms * 16 ? want : (u64)sms * 16);
+    zb_chain_index<<<grid, 256, 0, st>>>(src, (const ZeChainSeg*)segs, pos_off, n_segs);
+}
+void zb_launch_compress_chain_blocks(const u8* src, const void* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes,
+                                     void* outs, u32* work_counter, const void* segs, cudaStream_t st)
+{
+    ZeDict dict; memset(&dict, 0, sizeof dict); dict.cct = segs;
+    ZeUpload up; up.progress = nullptr; up.total = 0; up.status = nullptr;
+    cudaFuncSetAttribute(zb_compress_blocks<false, ZE_UNIT, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ZeShared));
+    zb_compress_blocks<false, ZE_UNIT, false, true><<<n_ctas, ZE_THREADS, sizeof(ZeShared), st>>>(src, (const ZeBlockJob*)jobs, n_jobs, (ZeScratch*)scratch,
+                                                                                            slots, slot_bytes, (ZeBlockOut*)outs, work_counter, dict, up, nullptr);
 }
 
 void zb_launch_frame_layout(const ZbSegment* segs, const void* seginfo, const void* outs, u32 n_segs, u32 checksum, u32 content_size,

@@ -212,7 +212,11 @@ int zb200_train_dictionary(zb200_ctx* ctx, const void* samples, const size_t* si
 const void*          zb200_result_data(const zb200_result* r);       /* host (pinned; pageable for zb200_compress_chain) or device pointer */
 uint64_t             zb200_result_size(const zb200_result* r);       /* bytes in data */
 size_t               zb200_result_count(const zb200_result* r);
-const zb200_segment* zb200_result_segments(const zb200_result* r);   /* host array, count entries */
+/* host array, count entries, valid until zb200_result_free.  A decode result copies its table into pinned memory of the
+ * context's pool; one that stays on the device (ZB200_DST_DEVICE) keeps the table on the device until the first call of
+ * this function, which copies it and waits for the copy (later calls return the same array).  NULL if that copy fails
+ * (zb200_ctx_last_error says why). */
+const zb200_segment* zb200_result_segments(const zb200_result* r);
 /* first failing item (lowest index wins, like the reference's worker error scan):
  * returns 0 if every item succeeded, else 1 and fills item/code/got/expected */
 int  zb200_result_first_error(const zb200_result* r, size_t* item, int* code, uint64_t* got, uint64_t* expected);

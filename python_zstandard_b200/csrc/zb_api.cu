@@ -155,7 +155,13 @@ struct zb200_result {
     bool data_owned_device = false;        // ZB200_DST_DEVICE: the result owns its device allocation (stream-ordered pool)
     std::vector<u8> host_data;             // zb200_compress_chain: the frames, in pageable memory the result owns
     u64 size = 0; size_t n = 0;
-    std::vector<zb200_segment> segs;
+    std::vector<zb200_segment> segs;       // compress and chain results: the table in pageable memory the result owns
+    // batch decode: the table in a block of the context's pinned pool.  A device-resident result (ZB200_DST_DEVICE) keeps
+    // its table in a device allocation of its own (stream-ordered pool) and copies it here on the first
+    // zb200_result_segments: a caller that never reads it pays no device->host copy
+    mutable zb200_segment* segs_pinned = nullptr;
+    ZbSegment* segs_device = nullptr;
+    mutable std::mutex segs_mu;
     bool has_error = false; size_t err_item = 0; int err_code = 0; u64 err_got = 0, err_expected = 0;
 };
 
@@ -509,7 +515,6 @@ static int run_decompress(zb200_ctx* ctx, const u8* d_src, const ZbSegment* d_se
                                    ctx->status.as<u32>(), ctx->out_sizes.as<u64>(), ctx->ck.as<u32>(), ctx->erep.as<u32>(), ctx->stream, chain != nullptr); }
     }
     res->n = n; res->size = totals[0];
-    res->segs.resize(n);
     if (copy_back) {
         res->data = pinned_get(ctx, totals[0] ? totals[0] : 1);
         if (!res->data) return fail(ctx, "pinned output allocation", cudaErrorMemoryAllocation);
@@ -555,11 +560,23 @@ static int run_decompress(zb200_ctx* ctx, const u8* d_src, const ZbSegment* d_se
             if (o1 > o0) CK(cudaMemcpyAsync((u8*)res->data + o0, d_out + o0, o1 - o0, cudaMemcpyDeviceToHost, ctx->copy_stream));
         }
     }
+    // The segment table.  Its memory is taken only now, with the decode kernels queued: nothing they do not need runs while
+    // the device waits.  A result that stays on the device keeps its table in an allocation of its own (stream-ordered
+    // pool) until the caller asks for it (zb200_result_segments); the others copy it into a block of the pinned pool.
+    ZbSegment* d_table = ctx->out_segs.as<ZbSegment>();
+    if (res->data_owned_device) {
+        void* p = nullptr; CK(cudaMallocAsync(&p, n * sizeof(ZbSegment), ctx->stream));
+        d_table = (ZbSegment*)p; res->segs_device = d_table;
+    }
     { KSpan s(ctx, ZB200_K_FINISH);
       zb_launch_finish(ctx->place.as<ZbFramePlace>(), ctx->out_sizes.as<u64>(), ctx->status.as<u32>(), nf,
-                       ctx->out_segs.as<ZbSegment>(), d_first_err, ctx->stream); }
+                       d_table, d_first_err, ctx->stream); }
+    if (!res->segs_device) {
+        res->segs_pinned = (zb200_segment*)pinned_get(ctx, n * sizeof(ZbSegment));
+        if (!res->segs_pinned) return fail(ctx, "pinned segment table", cudaErrorMemoryAllocation);
+        CK(cudaMemcpyAsync(res->segs_pinned, d_table, n * sizeof(ZbSegment), cudaMemcpyDeviceToHost, ctx->stream));
+    }
     u32 first_err = 0xFFFFFFFFu;
-    CK(cudaMemcpyAsync(res->segs.data(), ctx->out_segs.p, n * sizeof(ZbSegment), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaMemcpyAsync(&first_err, d_first_err, sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
     if (copy_back && n_chunks == 1) CK(cudaMemcpyAsync(res->data, d_out, totals[0], cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
@@ -766,7 +783,7 @@ int zb200_decompress_chain(zb200_ctx* ctx, const void* const* srcs, const size_t
         cudaError_t e = cudaSuccess;
         if (!rc && rr->has_error) chunk_error(k + rr->err_item, rr->err_code);
         else if (!rc) {         // the run's last fulltext becomes the next prefix
-            zb200_segment const last = rr->segs[b - k - 1];
+            zb200_segment const last = rr->segs_pinned[b - k - 1];
             carry = last.length;
             if (carry) e = ctx->carry.ensure(carry);
             if (carry && e == cudaSuccess) e = cudaMemcpyAsync(ctx->carry.p, ctx->dst.as<u8>() + last.offset, carry, cudaMemcpyDeviceToDevice, ctx->stream);
@@ -1131,7 +1148,25 @@ uint64_t zb200_compress_bound(uint64_t n) { return n + (n >> 8) + (n < (128u << 
 const void* zb200_result_data(const zb200_result* r) { return r->data; }
 uint64_t zb200_result_size(const zb200_result* r) { return r->size; }
 size_t zb200_result_count(const zb200_result* r) { return r->n; }
-const zb200_segment* zb200_result_segments(const zb200_result* r) { return r->segs.data(); }
+const zb200_segment* zb200_result_segments(const zb200_result* r)
+{
+    if (!r->segs_device) return r->segs_pinned ? r->segs_pinned : r->segs.data();
+    // a device-resident decode result: its table comes to the host on the first read.  The call that made the result
+    // synchronised its stream, so the table is complete; the copy goes on the copy stream, not behind later calls' kernels
+    std::lock_guard<std::mutex> g(r->segs_mu);
+    if (!r->segs_pinned) {
+        zb200_ctx* const ctx = r->ctx;
+        cudaSetDevice(ctx->device);
+        size_t const bytes = r->n * sizeof(zb200_segment);
+        auto* h = (zb200_segment*)pinned_get(ctx, bytes);
+        if (!h) { fail(ctx, "pinned segment table", cudaErrorMemoryAllocation); return nullptr; }
+        cudaError_t e = cudaMemcpyAsync(h, r->segs_device, bytes, cudaMemcpyDeviceToHost, ctx->copy_stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->copy_stream);
+        if (e != cudaSuccess) { pinned_put(ctx, h); fail(ctx, "zb200_result_segments", e); return nullptr; }
+        r->segs_pinned = h;
+    }
+    return r->segs_pinned;
+}
 int zb200_result_first_error(const zb200_result* r, size_t* item, int* code, uint64_t* got, uint64_t* expected)
 {
     if (!r->has_error) return 0;
@@ -1142,7 +1177,9 @@ void zb200_result_free(zb200_result* r)
 {
     if (!r) return;
     if (r->data && r->data_pinned_pool) pinned_put(r->ctx, r->data);
+    if (r->segs_pinned) pinned_put(r->ctx, r->segs_pinned);
     if (r->data && r->data_owned_device) { cudaSetDevice(r->ctx->device); cudaFreeAsync(r->data, r->ctx->stream); }
+    if (r->segs_device) { cudaSetDevice(r->ctx->device); cudaFreeAsync(r->segs_device, r->ctx->stream); }
     delete r;
 }
 

@@ -925,7 +925,7 @@ zb_execute(const u8* __restrict__ src, const ZbFramePlace* __restrict__ place, c
 // ---------------------------------------------------------------------------
 #define ZB_TILE_CAP    4096
 #define ZB_TILE_WARPS  8
-#define ZB_TILE_WARP_BYTES (2 * ZB_TILE_CAP + 64)
+#define ZB_TILE_WARP_BYTES (ZB_TILE_CAP + 64)     // output tile at the frame's 16-byte phase; its literals are staged inside it
 #define ZB_TILE_SMEM   (ZB_TILE_WARPS * ZB_TILE_WARP_BYTES)
 
 // per-phase cycle counters of zb_execute_tile (lane 0 of every warp) exist only in tuning builds (-DZB_PHASE_TIMERS):
@@ -941,7 +941,9 @@ __device__ unsigned long long g_zb_exe_phase[4];
 #define ZB_XFLUSH() do { } while (0)
 #endif
 
-__global__ void __launch_bounds__(ZB_TILE_WARPS * 32)
+// 5 CTAs per SM (40 warps; shared memory would allow 6): 48 registers.  Left to itself ptxas takes 62 and fits 4 CTAs,
+// which measured slower (DESIGN §4, K4).
+__global__ void __launch_bounds__(ZB_TILE_WARPS * 32, 5)
 zb_execute_tile(const u8* __restrict__ src, const ZbFramePlace* __restrict__ place, const u32* __restrict__ status,
                 const ZbBlock* __restrict__ blocks, const ZbSeq* __restrict__ seqs, const u8* __restrict__ lits,
                 u8* __restrict__ dst, u32 first, u32 n_frames, ZbDictDev dict)
@@ -957,10 +959,20 @@ zb_execute_tile(const u8* __restrict__ src, const ZbFramePlace* __restrict__ pla
     u64 const blk_end = place[f + 1].blk_off;
     u32 const skew = (u32)(pl.dst_off & 15);             // same 16-byte phase in smem as in dst
     u8* const so = zb_tile + warp * ZB_TILE_WARP_BYTES + skew;          // output tile
-    u8* const sl = zb_tile + warp * ZB_TILE_WARP_BYTES + ZB_TILE_CAP + 32;   // literal tile (16-byte aligned)
     const u8* const dict_end = dict.content + dict.content_size;
     u32 total = 0;
 
+    // Literals are staged IN PLACE, at sl = align16(so + dst_cap - n_lit) inside the output tile.  Literal j of a block goes
+    // to out_pos + j + M(j), M(j) = the block's match bytes in front of it, and out_pos + regen <= dst_cap with regen =
+    // n_lit + all the block's match bytes, so every literal's output lies at or below its staged copy: P(j) <= sl + j.
+    // Hence nothing written for literals up to j reaches a staged literal after j: match copies of a group end below the
+    // next group's literals, literal runs and the block's last literals are copied forward with loads ahead of stores
+    // (destination <= source), and the next block stages its literals above everything written so far.  The one hazard
+    // is INSIDE a group's literal copies, which run side by side: a later lane's run may land on an earlier lane's
+    // staged literals before that lane has read them.  A group whose runs all end at or below its lowest staged literal
+    // copies lane by lane as usual; any other group copies its literals as one stream, in warp-wide steps that load
+    // before they store, so each step writes only below what later steps read.  Rounding sl up only adds margin; the
+    // 16-byte staging over-read ends at most 30 bytes past dst_cap, inside the warp's slice.
     for (u64 bi = pl.blk_off; bi < blk_end; bi++) {
         ZbBlock const B = blocks[bi];
         u8* const bout = so + B.out_pos;
@@ -969,6 +981,8 @@ zb_execute_tile(const u8* __restrict__ src, const ZbFramePlace* __restrict__ pla
         if (B.kind == ZB_BLK_RLE) { for (u32 i = lane; i < B.regen; i += 32) bout[i] = (u8)B.lit_byte; __syncwarp(); ZB_XMARK(0); continue; }
         if (B.kind != ZB_BLK_COMPRESSED) return;
         bool const lit_rle = B.lit_kind == ZB_LIT_RLE; u8 const lit_byte = (u8)B.lit_byte;
+        u32 const lrel = (((u32)(uintptr_t)(so + pl.dst_cap - B.n_lit) + 15) & ~15u) - (u32)(uintptr_t)so;
+        u8* const sl = so + lrel;
         if (B.lit_kind == ZB_LIT_SCRATCH) {               // 16-byte aligned slice of the literal scratch
             const uint4* g = (const uint4*)(lits + B.src_pos); uint4* d4 = (uint4*)sl;
             for (u32 i = lane; i < (B.n_lit + 15) / 16; i += 32) d4[i] = g[i];
@@ -986,10 +1000,28 @@ zb_execute_tile(const u8* __restrict__ src, const ZbFramePlace* __restrict__ pla
             if (lane == 31 || i + 1 >= nseq) nx = valid ? sq[i + 1].x : 0;
             u32 const ll = nx - r.x, ml = r.z, off = r.w;
             u32 const ostart = r.y, mstart = r.y + ll;
-            if (valid) {
-                u8* o = bout + ostart;
-                if (lit_rle) for (u32 k = 0; k < ll; k++) o[k] = lit_byte;
-                else zb_copy_fwd8(o, sl + r.x, ll);
+            u32 const x0 = __shfl_sync(0xFFFFFFFFu, r.x, 0);
+            if (lit_rle || !__any_sync(0xFFFFFFFFu, valid && (u32)B.out_pos + mstart > lrel + x0)) {
+                if (valid) {
+                    u8* o = bout + ostart;
+                    if (lit_rle) for (u32 k = 0; k < ll; k++) o[k] = lit_byte;
+                    else zb_copy_fwd8(o, sl + r.x, ll);         // destination <= source: each 8-byte chunk loads first
+                }
+            } else {
+                // literal j of the group goes to bout + ostart_s + j - x_s for the last lane s with x_s <= j
+                u32 const xe = __shfl_sync(0xFFFFFFFFu, nx, min(31u, nseq - 1 - g));
+                u32 const key = valid ? r.x : 0xFFFFFFFFu;
+                int const delta = (int)ostart - (int)r.x;
+                for (u32 j0 = x0; j0 < xe; j0 += 32) {
+                    u32 const j = j0 + lane;
+                    u32 s = 0;                                   // lane 0 (key x0 <= j) qualifies
+                    for (u32 b = 16; b; b >>= 1) if (__shfl_sync(0xFFFFFFFFu, key, s + b) <= j) s += b;
+                    int const dj = __shfl_sync(0xFFFFFFFFu, delta, (int)s);
+                    u8 const v = j < xe ? sl[j] : 0;
+                    __syncwarp();
+                    if (j < xe) bout[(int)j + dj] = v;
+                    __syncwarp();
+                }
             }
             __syncwarp();
             ZB_XMARK(1);
@@ -1048,7 +1080,14 @@ zb_execute_tile(const u8* __restrict__ src, const ZbFramePlace* __restrict__ pla
             ZbSeq const e = sq[nseq];
             u32 const tail = B.n_lit - e.x;
             if (lit_rle) { for (u32 k = lane; k < tail; k += 32) bout[e.y + k] = lit_byte; }
-            else for (u32 k = lane; k < tail; k += 32) bout[e.y + k] = sl[e.x + k];
+            else
+                for (u32 k0 = 0; k0 < tail; k0 += 32) {           // in place (destination <= source): load, then store
+                    u32 const k = k0 + lane;
+                    u8 const v = k < tail ? sl[e.x + k] : 0;
+                    __syncwarp();
+                    if (k < tail) bout[e.y + k] = v;
+                    __syncwarp();
+                }
         }
         __syncwarp();
         ZB_XMARK(1);

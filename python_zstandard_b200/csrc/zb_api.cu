@@ -827,9 +827,7 @@ static int compress_common(zb200_ctx* ctx, const void* src_base, const zb200_seg
     double const tr0 = zb_trace_on() ? zb_now_ms() : 0; double tr1 = 0, tr2 = 0;
     zb200_cparams P; if (params) P = *params; else { memset(&P, 0, sizeof P); P.level = 3; P.write_content_size = 1; }
     if (P.window_log && (P.window_log < 10 || P.window_log > 31)) return fail(ctx, "zb200_compress_batch: window_log out of range [10, 31]", cudaSuccess);
-    // Block_Maximum_Size = min(window, 128 KiB) (ZSTD_getBlockSize, zstd/zstd.c:27478): a small window cuts the blocks, and with
-    // them the reach of every match (matches never leave their block here)
-    u32 const block_max = P.window_log && P.window_log < 17 ? (1u << P.window_log) : ZB_BLOCK_MAX;
+    u32 const block_max = zb_block_max(P.window_log);
     std::vector<zb200_segment> hsegs;
     const u8* d_src; const ZbSegment* d_segs;
     const u8* up_src = nullptr; u64 up_bytes = 0;          // host input to upload while the kernel runs
@@ -859,20 +857,9 @@ static int compress_common(zb200_ctx* ctx, const void* src_base, const zb200_seg
         d_src = ctx->src.as<u8>(); d_segs = ctx->segs.as<ZbSegment>();
     }
     if (zb_trace_on()) tr1 = zb_now_ms();
-    // block jobs: every <=128 KiB slice of every segment (ZSTD_compress_frameChunk's block loop, zstd/zstd.c:27545)
     std::vector<HostJob> jobs; std::vector<HostSegInfo> sinfo(n);
     jobs.reserve(n);
-    u32 max_block = 0;
-    for (size_t i = 0; i < n; i++) {
-        u64 const len = hsegs[i].length; u64 pos = 0;
-        sinfo[i].first_job = jobs.size(); sinfo[i].n_jobs = 0; sinfo[i].pad = 0;
-        while (pos < len) {
-            u32 const sz = (u32)(len - pos < block_max ? len - pos : block_max);
-            HostJob j; j.src_pos = hsegs[i].offset + pos; j.size = sz; j.seg = (u32)i; j.first = pos == 0; j.last = pos + sz == len;
-            jobs.push_back(j); sinfo[i].n_jobs++; pos += sz;
-            if (sz > max_block) max_block = sz;
-        }
-    }
+    u32 const max_block = zb_cut_blocks(hsegs.data(), n, block_max, jobs, sinfo);
     size_t const nj = jobs.size();
     u64 const slot_bytes = ((u64)max_block + (max_block >> 7) + 64 + 15) & ~15ull;
     // Blocks of 8 KiB and more (no dictionary, level-3 class) take the round-2 kernel: one CTA per SM with the block resident in

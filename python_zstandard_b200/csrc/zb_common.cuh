@@ -43,6 +43,32 @@ enum : u32 {
 
 struct ZbSegment { u64 offset, length; };       // == BufferSegment, c-ext/python-zstandard.h:307-313
 
+// Block_Maximum_Size = min(window, 128 KiB) (ZSTD_getBlockSize, zstd/zstd.c:27478): a window_log below 17 cuts blocks of
+// 2^window_log bytes, and with them the reach of every match; 0 = the default window
+static inline u32 zb_block_max(u32 window_log) { return window_log && window_log < 17 ? (1u << window_log) : ZB_BLOCK_MAX; }
+
+// The block jobs of a compression call: every <= block_max slice of every segment (ZSTD_compress_frameChunk's block loop,
+// zstd/zstd.c:27545), in segment order, so a job that is not the first of its frame comes right after the one in front of
+// it.  Host code; the launcher and the CPU build of the kernels both cut their jobs here, each with its own structs of the
+// same fields.  Returns the largest block.
+template <class Seg, class JobVec, class InfoVec>
+static inline u32 zb_cut_blocks(const Seg* segs, size_t n, u32 block_max, JobVec& jobs, InfoVec& info)
+{
+    u32 max_block = 0;
+    for (size_t i = 0; i < n; i++) {
+        u64 const len = segs[i].length; u64 pos = 0;
+        info[i].first_job = jobs.size(); info[i].n_jobs = 0; info[i].pad = 0;
+        while (pos < len) {
+            u32 const sz = (u32)(len - pos < block_max ? len - pos : block_max);
+            typename JobVec::value_type j;
+            j.src_pos = segs[i].offset + pos; j.size = sz; j.seg = (u32)i; j.first = pos == 0; j.last = pos + sz == len;
+            jobs.push_back(j); info[i].n_jobs++; pos += sz;
+            if (sz > max_block) max_block = sz;
+        }
+    }
+    return max_block;
+}
+
 // result of the frame scan (one per frame)
 struct ZbFrameInfo {
     u64 content_size;     // from the header, ZB_CONTENT_UNKNOWN if absent

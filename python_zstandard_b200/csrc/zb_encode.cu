@@ -625,10 +625,14 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
         long long t_phase = clock64();
         const u8* const in = src + job.src_pos;
         // bytes of history in front of the block: the dictionary tail for the first block of a frame; in the two-table mode the
-        // last ZE_HIST bytes of the previous block for the others (it is a full 128 KiB block of the same frame, so it sits
-        // right in front of `in`); otherwise blocks are compressed independently
+        // last ZE_HIST bytes of the previous block for the others when that block holds at least 64 KiB; otherwise blocks are
+        // compressed independently.  The previous job is the block in front of this one in the same frame (zb_cut_blocks), and
+        // a block that is not its frame's last one is a full block_max = min(2^window_log, 128 KiB) bytes.  So the history sits
+        // inside the frame, and the window is at least 64 KiB, which every offset here stays below (u16 distances).  Blocks
+        // cut smaller by window_log < 16 get none: in front of a 1 .. 16 KiB block, 32 KiB would reach out of the frame, and
+        // in front of a 32 KiB block the matches would reach up to 64 KiB back through a 32 KiB window.
         constexpr u32 ZE_HIST = 32768;
-        bool const hist = DUAL && !job.first;
+        bool const hist = DUAL && !job.first && jobs[j - 1].size >= 65536u;
         ZeChainSeg cs = {}; if constexpr (PREFIX) cs = ((const ZeChainSeg*)dict.cct)[job.seg];
         u32 const bpos = PREFIX ? (u32)(job.src_pos - cs.start) : 0u;             // (PREFIX) block position in its chunk
         // PREFIX: everything in front of the block back to the start of the previous chunk is history

@@ -148,7 +148,7 @@ def first_frame(chunk, checksum=False, dict_data=None):
     o_off, o_len = np.zeros(1, np.uint64), np.zeros(1, np.uint64)
     d = bytes(dict_data) if dict_data else None
     n = _batch.t_compress_batch(data.ctypes.data, off.ctypes.data, ln.ctypes.data, 1, int(checksum), 1, 4, out.ctypes.data, cap,
-                                o_off.ctypes.data, o_len.ctypes.data, 0, d, len(d) if d else 0)
+                                o_off.ctypes.data, o_len.ctypes.data, 0, d, len(d) if d else 0, 3, 0)
     assert n > 0, n
     return out[int(o_off[0]):int(o_off[0] + o_len[0])].tobytes()
 

@@ -157,22 +157,18 @@ def build_header_parser():
 SIM_LIB = os.path.join(BUILD, "libzs_host.so")
 SIM_WRAPPERS = r"""
 extern "C" unsigned long long t_any_calls(int reset) { unsigned long long v = simt_any_calls; if (reset) simt_any_calls = 0; return v; }
-// The whole compression path of the library on the CPU: block jobs as zb_api.cu makes them, zb_compress_blocks on
-// `n_ctas` CTAs of 128 threads, then the frame layout kernels.  No dictionary, input resident.  Returns total bytes.
+// The whole compression path of the library on the CPU: block jobs cut as zb_api.cu cuts them (zb_cut_blocks, blocks of
+// min(2^window_log, 128 KiB)), zb_compress_blocks on `n_ctas` CTAs of 128 threads -- the two-table instantiation from level 4
+// on, as the launcher picks it -- or zb_compress_recs when `recs` is set, then the frame layout kernels with the level and
+// window_log of the call.  Input resident.  Returns total bytes.
 extern "C" long long t_compress_batch(const u8* src, const u64* seg_off, const u64* seg_len, u32 n_segs, u32 checksum, u32 content_size,
-                                      u32 n_ctas, u8* out, u64 out_cap, u64* out_off, u64* out_len, u32 dual, const u8* dict_raw, u32 dict_n)
+                                      u32 n_ctas, u8* out, u64 out_cap, u64* out_off, u64* out_len, u32 recs, const u8* dict_raw, u32 dict_n,
+                                      int level, u32 window_log)
 {
     std::vector<ZbSegment> segs(n_segs); std::vector<ZeBlockJob> jobs; std::vector<ZeSegInfo> info(n_segs);
-    u32 max_block = 0;
-    for (u32 i = 0; i < n_segs; i++) {
-        segs[i].offset = seg_off[i]; segs[i].length = seg_len[i];
-        info[i].first_job = jobs.size(); info[i].n_jobs = 0; info[i].pad = 0;
-        for (u64 pos = 0; pos < seg_len[i];) {
-            u32 const sz = (u32)(seg_len[i] - pos < ZE_BLOCK ? seg_len[i] - pos : ZE_BLOCK);
-            ZeBlockJob j; j.src_pos = seg_off[i] + pos; j.size = sz; j.seg = i; j.first = pos == 0; j.last = pos + sz == seg_len[i];
-            jobs.push_back(j); info[i].n_jobs++; pos += sz; if (sz > max_block) max_block = sz;
-        }
-    }
+    for (u32 i = 0; i < n_segs; i++) { segs[i].offset = seg_off[i]; segs[i].length = seg_len[i]; }
+    u32 const max_block = zb_cut_blocks(segs.data(), n_segs, zb_block_max(window_log), jobs, info);
+    bool const dual = level >= 4;
     u32 const nj = (u32)jobs.size();
     u64 const slot_bytes = ((u64)max_block + (max_block >> 7) + 64 + 15) & ~15ull;
     std::vector<u8> slots((size_t)(nj + 1) * slot_bytes); std::vector<ZeBlockOut> outs(nj + 1);
@@ -195,9 +191,9 @@ extern "C" long long t_compress_batch(const u8* src, const u64* seg_off, const u
         }
     }
     ZeUpload up; up.progress = nullptr; up.total = 0; up.status = nullptr;
-    ZeParams P; P.checksum = checksum; P.content_size = content_size; P.dict_id = dict_id; P.level = 3;
+    ZeParams P; P.checksum = checksum; P.content_size = content_size; P.dict_id = dict_id; P.level = (u32)level; P.window_log = window_log;
     bool const small_blocks = max_block <= ZE_SMALL_MAX;             // as zb_api.cu picks the instantiation
-    if (nj && dual == 2) simt::launch((nj + Z3_WARPS - 1) / Z3_WARPS < n_ctas ? (nj + Z3_WARPS - 1) / Z3_WARPS : n_ctas, Z3_NT, [&] { zb_compress_recs(src, jobs.data(), nj, slots.data(), slot_bytes, outs.data(), &counter, dict, up); });
+    if (nj && recs) simt::launch((nj + Z3_WARPS - 1) / Z3_WARPS < n_ctas ? (nj + Z3_WARPS - 1) / Z3_WARPS : n_ctas, Z3_NT, [&] { zb_compress_recs(src, jobs.data(), nj, slots.data(), slot_bytes, outs.data(), &counter, dict, up); });
     else if (nj && dual && small_blocks) simt::launch(n_ctas, ZE_THREADS, [&] { zb_compress_blocks<true, ZE_UNIT_SMALL>(src, jobs.data(), nj, (ZeScratch*)scratch, slots.data(), slot_bytes, outs.data(), &counter, dict, up); });
     else if (nj && small_blocks) simt::launch(n_ctas, ZE_THREADS, [&] { zb_compress_blocks<false, ZE_UNIT_SMALL>(src, jobs.data(), nj, (ZeScratch*)scratch, slots.data(), slot_bytes, outs.data(), &counter, dict, up); });
     else if (nj && dual) simt::launch(n_ctas, ZE_THREADS, [&] { zb_compress_blocks<true, ZE_UNIT>(src, jobs.data(), nj, (ZeScratch*)scratch, slots.data(), slot_bytes, outs.data(), &counter, dict, up); });
@@ -212,21 +208,14 @@ extern "C" long long t_compress_batch(const u8* src, const u64* seg_off, const u
     return (long long)total;
 }
 
-// The round-2 kernel (zb_compress_smem: one CTA of 1024 threads per block, block resident in "shared memory") on the CPU.
+// The round-2 kernel (zb_compress_smem: one CTA of 1024 threads per block, block resident in "shared memory") on the CPU,
+// with the jobs and frame headers of a call with this level and window_log.
 extern "C" long long t_compress_batch2(const u8* src, const u64* seg_off, const u64* seg_len, u32 n_segs, u32 checksum, u32 content_size,
-                                       u32 n_ctas, u8* out, u64 out_cap, u64* out_off, u64* out_len)
+                                       u32 n_ctas, u8* out, u64 out_cap, u64* out_off, u64* out_len, int level, u32 window_log)
 {
     std::vector<ZbSegment> segs(n_segs); std::vector<ZeBlockJob> jobs; std::vector<ZeSegInfo> info(n_segs);
-    u32 max_block = 0;
-    for (u32 i = 0; i < n_segs; i++) {
-        segs[i].offset = seg_off[i]; segs[i].length = seg_len[i];
-        info[i].first_job = jobs.size(); info[i].n_jobs = 0; info[i].pad = 0;
-        for (u64 pos = 0; pos < seg_len[i];) {
-            u32 const sz = (u32)(seg_len[i] - pos < ZE_BLOCK ? seg_len[i] - pos : ZE_BLOCK);
-            ZeBlockJob j; j.src_pos = seg_off[i] + pos; j.size = sz; j.seg = i; j.first = pos == 0; j.last = pos + sz == seg_len[i];
-            jobs.push_back(j); info[i].n_jobs++; pos += sz; if (sz > max_block) max_block = sz;
-        }
-    }
+    for (u32 i = 0; i < n_segs; i++) { segs[i].offset = seg_off[i]; segs[i].length = seg_len[i]; }
+    u32 const max_block = zb_cut_blocks(segs.data(), n_segs, zb_block_max(window_log), jobs, info);
     u32 const nj = (u32)jobs.size();
     u64 const slot_bytes = ((u64)max_block + (max_block >> 7) + 64 + 15) & ~15ull;
     u8* slots = (u8*)aligned_alloc(64, (size_t)(nj + 1) * slot_bytes + 64); std::vector<ZeBlockOut> outs(nj + 1);
@@ -234,7 +223,7 @@ extern "C" long long t_compress_batch2(const u8* src, const u64* seg_off, const 
     Z2Scratch* scratch = (Z2Scratch*)aligned_alloc(64, ((sizeof(Z2Scratch) + 63) & ~(size_t)63) * n_ctas);
     u32 counter = 0;
     ZeUpload up; up.progress = nullptr; up.total = 0; up.status = nullptr;
-    ZeParams P; P.checksum = checksum; P.content_size = content_size; P.dict_id = 0; P.level = 3;
+    ZeParams P; P.checksum = checksum; P.content_size = content_size; P.dict_id = 0; P.level = (u32)level; P.window_log = window_log;
     if (nj) simt::launch(n_ctas, Z2_NT, [&] { zb_compress_smem(src, jobs.data(), nj, scratch, slots, slot_bytes, outs.data(), &counter, up); });
     std::vector<u64> sizes(n_segs); std::vector<ZbSegment> out_segs(n_segs); u64 total = 0;
     simt::launch((n_segs + 255) / 256, 256, [&] { zb_frame_sizes(segs.data(), info.data(), outs.data(), n_segs, P, sizes.data()); });
@@ -279,10 +268,11 @@ def build_compress_sim():
     L = C.CDLL(SIM_LIB)
     L.t_compress_batch.restype = C.c_longlong
     L.t_compress_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
-                                   C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
+                                   C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32,
+                                   C.c_int, C.c_uint32]
     L.t_compress_batch2.restype = C.c_longlong
     L.t_compress_batch2.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
-                                    C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]
+                                    C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_int, C.c_uint32]
     return L
 
 

@@ -31,8 +31,11 @@ def ref():
     return RefZstd()
 
 
-def compress(sim, segs, checksum=False, content_size=True, n_ctas=2, dual=False, dct=b""):
-    """[frame bytes] for a batch of byte strings through the kernel source."""
+def compress(sim, segs, checksum=False, content_size=True, n_ctas=2, dual=False, dct=b"", level=None, window_log=0):
+    """[frame bytes] for a batch of byte strings through the kernel source.  dual=True: the level >= 4 mode (level 4 unless
+    `level` says otherwise); dual=2: the record kernel zb_compress_recs.  window_log 0: the default window."""
+    if level is None:
+        level = 4 if dual is True or dual == 1 else 3
     blob = b"".join(segs) + bytes(64)
     off = np.cumsum([0] + [len(s) for s in segs[:-1]]).astype(np.uint64)
     ln = np.array([len(s) for s in segs], dtype=np.uint64)
@@ -42,8 +45,8 @@ def compress(sim, segs, checksum=False, content_size=True, n_ctas=2, dual=False,
     oo = (C.c_uint64 * len(segs))(); ol = (C.c_uint64 * len(segs))()
     dbuf = (C.c_ubyte * (len(dct) + 64)).from_buffer_copy(dct + bytes(64))
     tot = sim.t_compress_batch(C.addressof(src), off.ctypes.data, ln.ctypes.data, len(segs), int(checksum), int(content_size), n_ctas,
-                               C.addressof(out), cap, C.addressof(oo), C.addressof(ol), int(dual),
-                               C.addressof(dbuf) if dct else None, len(dct))
+                               C.addressof(out), cap, C.addressof(oo), C.addressof(ol), int(dual == 2),
+                               C.addressof(dbuf) if dct else None, len(dct), level, window_log)
     assert tot >= 0 and tot == sum(ol)
     assert all(oo[i] == sum(ol[:i]) for i in range(len(segs)))          # frames are packed tightly, in order
     return [bytes(out[oo[i]:oo[i] + ol[i]]) for i in range(len(segs))]
@@ -175,7 +178,7 @@ def test_two_table_mode_uses_the_previous_block_as_history(sim, ref):
 # The round-2 kernel (zb_compress_smem: one CTA of 1024 threads per block, the block resident in shared memory, serial hash
 # links beside warp-per-region verify + parse, sub-blocks with their FSE state chains side by side).  The launcher gives
 # it every call whose largest block is >= 8 KiB (no dictionary, level-3 class).
-def compress_smem(sim, segs, checksum=False, n_ctas=2):
+def compress_smem(sim, segs, checksum=False, n_ctas=2, content_size=True, level=3, window_log=0):
     blob = b"".join(segs) + bytes(64)
     off = np.cumsum([0] + [len(s) for s in segs[:-1]]).astype(np.uint64)
     ln = np.array([len(s) for s in segs], dtype=np.uint64)
@@ -183,8 +186,8 @@ def compress_smem(sim, segs, checksum=False, n_ctas=2):
     cap = sum(len(s) + len(s) // 128 + 64 for s in segs) + 64
     out = (C.c_ubyte * cap)()
     oo = (C.c_uint64 * len(segs))(); ol = (C.c_uint64 * len(segs))()
-    tot = sim.t_compress_batch2(C.addressof(src), off.ctypes.data, ln.ctypes.data, len(segs), int(checksum), 1, n_ctas,
-                                C.addressof(out), cap, C.addressof(oo), C.addressof(ol))
+    tot = sim.t_compress_batch2(C.addressof(src), off.ctypes.data, ln.ctypes.data, len(segs), int(checksum), int(content_size), n_ctas,
+                                C.addressof(out), cap, C.addressof(oo), C.addressof(ol), level, window_log)
     assert tot >= 0 and tot == sum(ol)
     return [bytes(out[oo[i]:oo[i] + ol[i]]) for i in range(len(segs))]
 

@@ -20,7 +20,7 @@ def build(tag, extra):
     subprocess.check_call(["g++", "-std=c++17", "-O1", "-shared", "-fPIC", "-I/usr/local/cuda/include"] + extra + ["-o", lib, cpp])
     L = C.CDLL(lib); L.t_compress_batch.restype = C.c_longlong; L.t_any_calls.restype = C.c_ulonglong
     L.t_compress_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p,
-                                   C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
+                                   C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_int, C.c_uint32]
     return L
 
 

@@ -14,7 +14,7 @@ from oracle import RefZstd
 import corpus, numpy as np
 ref=RefZstd()
 Lc=C.CDLL('/tmp/libzs_ubsan.so'); Lc.t_compress_batch.restype=C.c_longlong
-Lc.t_compress_batch.argtypes=[C.c_void_p,C.c_void_p,C.c_void_p,C.c_uint32,C.c_uint32,C.c_uint32,C.c_uint32,C.c_void_p,C.c_uint64,C.c_void_p,C.c_void_p,C.c_uint32,C.c_void_p,C.c_uint32]
+Lc.t_compress_batch.argtypes=[C.c_void_p,C.c_void_p,C.c_void_p,C.c_uint32,C.c_uint32,C.c_uint32,C.c_uint32,C.c_void_p,C.c_uint64,C.c_void_p,C.c_void_p,C.c_uint32,C.c_void_p,C.c_uint32,C.c_int,C.c_uint32]
 Ld=C.CDLL('/tmp/libzd_ubsan.so'); Ld.t_decompress_batch.restype=C.c_longlong
 Ld.t_decompress_batch.argtypes=[C.c_void_p,C.c_void_p,C.c_void_p,C.c_uint32,C.c_void_p,C.c_uint32,C.c_uint32,C.c_uint32,C.c_uint32,C.c_void_p,C.c_uint64,C.c_void_p,C.c_void_p,C.c_void_p,C.c_void_p]
 text=corpus.text_corpus(1<<20)

@@ -465,10 +465,10 @@ static int run_decompress(zb200_ctx* ctx, const u8* d_src, const ZbSegment* d_se
     else { void* p = nullptr; CK(cudaMallocAsync(&p, totals[0] + 64, ctx->stream)); d_out = (u8*)p; res->data = p; res->data_on_device = true; res->data_owned_device = true; }
     ctx->last_scratch = (totals[1] + 1) * sizeof(ZbBlock) + (totals[2] + 1) * sizeof(ZbSeq) + totals[3];
 
-    // ---- chunks of frames: the device->host copy of chunk k overlaps the kernels of chunk k+1
-    u32 n_chunks = 1;
-    if (copy_back) { u64 c = totals[0] / (48ull << 20); n_chunks = (u32)(c < 1 ? 1 : (c > 32 ? 32 : c)); if (n_chunks > nf) n_chunks = nf; }
-    std::vector<u32> cut(n_chunks + 1); for (u32 k = 0; k <= n_chunks; k++) cut[k] = (u32)((u64)nf * k / n_chunks);
+    // ---- chunks of frames: the device->host copy of chunk k overlaps the kernels of chunk k+1 (zb_chunk_count)
+    u64 const chunk_bytes = getenv("ZB200_OUT_CHUNK_BYTES") ? strtoull(getenv("ZB200_OUT_CHUNK_BYTES"), nullptr, 10) : 0;   // (read per call: tests switch it)
+    u32 const n_chunks = zb_chunk_count(totals[0], nf, copy_back, chunk_bytes);
+    std::vector<u32> cut(n_chunks + 1); for (u32 k = 0; k <= n_chunks; k++) cut[k] = zb_chunk_cut(nf, k, n_chunks);
     std::vector<ZbFramePlace> cpl(n_chunks + 1);
     if (n_chunks > 1) {
         for (u32 k = 0; k <= n_chunks; k++)
@@ -523,17 +523,11 @@ static int run_decompress(zb200_ctx* ctx, const u8* d_src, const ZbSegment* d_se
     for (u32 k = 0; k < n_chunks; k++) {
         u32 const f0 = cut[k], f1 = cut[k + 1];
         u32* const counter = n_chunks > 1 ? d_counter + 8 + k : d_counter;
-        // frames per warp: large frames carry large decode tables (a 128 KiB block: ~4 KB Huffman + ~5 KB FSE cells per lane)
-        u64 const avg_out = (cpl.size() > 1 && n_chunks > 1 ? (cpl[k + 1].dst_off - cpl[k].dst_off) : totals[0]) / (f1 - f0 ? f1 - f0 : 1);
-        u32 const EW = avg_out <= (8u << 10) ? 8u : 7u;          // warps per CTA: see zb_entropy.cuh
-        u32 take = avg_out <= (8u << 10) ? 32u : (avg_out <= (16u << 10) ? 16u : (avg_out <= (32u << 10) ? 8u : (avg_out <= (64u << 10) ? 4u : 3u)));
-        // small batches: spread the frames over all resident warps rather than filling few warps' lanes
-        { u32 const spread = (f1 - f0 + ctas * EW - 1) / (ctas * EW); if (take > spread) take = spread ? spread : 1; }
-        u32 cc = ctas; { u32 const need = (f1 - f0 + EW * take - 1) / (EW * take); if (cc > need) cc = need; if (cc == 0) cc = 1; }
         if (!block_path) { KSpan s(ctx, ZB200_K_ENTROPY);
+          ZbChunkShape const sh = zb_chunk_shape(n_chunks > 1 ? cpl[k + 1].dst_off - cpl[k].dst_off : totals[0], f1 - f0, ctas);
           zb_launch_entropy(d_src, d_segs, f1, ctx->place.as<ZbFramePlace>(), exact_sizes ? d_dst_sizes : nullptr, ctx->blocks.as<ZbBlock>(),
-                            ctx->seqs.as<ZbSeq>(), ctx->lits.as<u8>(), cc, counter, dd,
-                            ctx->status.as<u32>(), ctx->out_sizes.as<u64>(), ctx->ck.as<u32>(), take, EW, ctx->stream); }
+                            ctx->seqs.as<ZbSeq>(), ctx->lits.as<u8>(), sh.ctas, counter, dd,
+                            ctx->status.as<u32>(), ctx->out_sizes.as<u64>(), ctx->ck.as<u32>(), sh.take, sh.warps, ctx->stream); }
         { KSpan s(ctx, ZB200_K_EXECUTE);
           if (chase_path) {
               int const r = zb_launch_execute_chase(d_src, ctx->place.as<ZbFramePlace>(), ctx->status.as<u32>(), ctx->blocks.as<ZbBlock>(), ctx->bdesc.p,

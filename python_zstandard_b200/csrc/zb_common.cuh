@@ -69,6 +69,38 @@ static inline u32 zb_cut_blocks(const Seg* segs, size_t n, u32 block_max, JobVec
     return max_block;
 }
 
+// The output chunks of a batch decode (run_decompress, zb_api.cu): a call whose output is copied back to the host is cut
+// into chunks of frames, and the copy of chunk k overlaps the kernels of chunk k + 1.  One chunk per `chunk_bytes` of
+// output, at most 32 and never more than there are frames; the cuts are by frame count (cut k = n_frames * k / n_chunks),
+// not by bytes, so every chunk holds at least one frame.  Host code; the launcher and the CPU build of the kernels both
+// plan their chunks here.
+#define ZB_OUT_CHUNK_BYTES (48ull << 20)
+#define ZB_OUT_CHUNKS_MAX  32u
+static inline u32 zb_chunk_count(u64 total_out, u32 n_frames, bool copy_back, u64 chunk_bytes)
+{
+    if (!copy_back || n_frames == 0) return 1;
+    u64 const c = total_out / (chunk_bytes ? chunk_bytes : ZB_OUT_CHUNK_BYTES);
+    u32 const k = (u32)(c < 1 ? 1 : (c > ZB_OUT_CHUNKS_MAX ? ZB_OUT_CHUNKS_MAX : c));
+    return k > n_frames ? n_frames : k;
+}
+static inline u32 zb_chunk_cut(u32 n_frames, u32 k, u32 n_chunks) { return (u32)((u64)n_frames * k / n_chunks); }
+
+// The lane-per-frame entropy launch of one chunk, from its output bytes, its frame count and the SM count: warps per CTA,
+// frames per warp and CTAs of the persistent grid.  Large frames carry large decode tables (a 128 KiB block: ~4 KB Huffman
+// + ~5 KB FSE cells per lane), so fewer of them share a warp (zb_entropy.cuh); small chunks spread their frames over all
+// resident warps rather than filling few warps' lanes.
+struct ZbChunkShape { u32 warps, take, ctas; };
+static inline ZbChunkShape zb_chunk_shape(u64 out_bytes, u32 n_frames, u32 sm_count)
+{
+    u64 const avg_out = out_bytes / (n_frames ? n_frames : 1);
+    ZbChunkShape s;
+    s.warps = avg_out <= (8u << 10) ? 8u : 7u;
+    s.take = avg_out <= (8u << 10) ? 32u : (avg_out <= (16u << 10) ? 16u : (avg_out <= (32u << 10) ? 8u : (avg_out <= (64u << 10) ? 4u : 3u)));
+    { u32 const spread = (n_frames + sm_count * s.warps - 1) / (sm_count * s.warps); if (s.take > spread) s.take = spread ? spread : 1; }
+    s.ctas = sm_count; { u32 const need = (n_frames + s.warps * s.take - 1) / (s.warps * s.take); if (s.ctas > need) s.ctas = need; if (s.ctas == 0) s.ctas = 1; }
+    return s;
+}
+
 // result of the frame scan (one per frame)
 struct ZbFrameInfo {
     u64 content_size;     // from the header, ZB_CONTENT_UNKNOWN if absent

@@ -296,9 +296,25 @@ extern "C" void t_scan_totals(const u8* src, const u64* seg_off, const u64* seg_
     simt::launch(pctas, ZB_PLACE_CTA, [&] { zb_place_scan(info.data(), nullptr, n, partial.data(), place.data(), totals, status.data()); });
     for (int k = 0; k < 6; k++) totals_out[k] = totals[k];
 }
+// `chunk_bytes` 0: one chunk of all frames, the entropy kernel on `n_ctas` CTAs of `warps` warps with `take` frames per warp.
+// Otherwise the call is cut as run_decompress cuts a call whose output is copied back (zb_chunk_count with this chunk size,
+// zb_chunk_cut), and every chunk runs what the launcher runs for it: the lane-per-frame entropy kernel over frames
+// [0, cut[k + 1]) from a counter of its own that starts at cut[k], shaped by zb_chunk_shape from the chunk's output bytes
+// with `n_ctas` as the SM count (the block path keeps its one entropy launch for all blocks); then the chunk's execute stage
+// -- zb_execute_tile + zb_execute over its frames, zb_execute_big over its blocks with a fresh wave, or the pointer-jumping
+// rounds over its output bytes -- and its checksums.  The pointer-jumping stage regenerates every frame itself, small ones
+// included: as in zb_launch_execute_chase, no tile executor runs in front of it.
+// The copy of chunk k overlaps the kernels of chunk k + 1 on the device.  Here the chunk's output range is copied into `out`
+// as soon as its kernels are done, and is then overwritten in the working buffer with bytes that differ from every output
+// byte (the copy may read at any moment, and no kernel of a later chunk may read or write there).  `out` holds nothing but
+// these copies.  The chunk's regenerated sizes are set aside the same way until zb_finish: a later chunk must not decode
+// its frames again.  plan (nullable, 3 + 5 * 33 words): n_chunks, bytes of earlier chunks that later chunks wrote, frames
+// of earlier chunks that later chunks decoded again; then per chunk {cut, warps, take, ctas, output bytes}, where warps, take
+// and ctas are those of the chunk's lane-per-frame entropy launch (0 on the block path, whose one launch is not per chunk).
 extern "C" long long t_decompress_batch(const u8* src, const u64* seg_off, const u64* seg_len, u32 n, const u8* dict_raw, u32 dict_n,
                                         u32 n_ctas, u32 warps, u32 take, u8* out, u64 out_cap, u64* out_off, u64* out_len, u32* status_out,
-                                        const u64* dst_sizes /* nullable: the decompressed_sizes argument of the batch call */)
+                                        const u64* dst_sizes /* nullable: the decompressed_sizes argument of the batch call */,
+                                        u64 chunk_bytes, u64* plan)
 {
     static bool tables = false;
     if (!tables) { simt::launch(1, 32, [] { zb_build_default_tables(); }); tables = true; }
@@ -323,35 +339,69 @@ extern "C" long long t_decompress_batch(const u8* src, const u64* seg_off, const
     simt::launch(pctas, ZB_PLACE_CTA, [&] { zb_place_scan(info.data(), dst_sizes, n, partial.data(), place.data(), totals, status.data()); });
     if (totals[0] > out_cap) return -1000;
     std::vector<ZbBlock> blocks(totals[1] + 1); std::vector<ZbSeq> seqs(totals[2] + 2); std::vector<u8> lits(totals[3] + 64);
-    std::vector<u64> out_sizes(n, 0); std::vector<u32> ck(n, 0); u32 counter = 0;
+    std::vector<u64> out_sizes(n, 0); std::vector<u32> ck(n, 0);
+    std::vector<u8> dev(totals[0] + 64, 0); u8* const d_out = dev.data();       // the device's output buffer
     std::vector<ZbBlkDesc> bdesc;
+    u32 const n_chunks = chunk_bytes ? zb_chunk_count(totals[0], n, true, chunk_bytes) : 1;
+    std::vector<u32> cut(n_chunks + 1); for (u32 k = 0; k <= n_chunks; k++) cut[k] = zb_chunk_cut(n, k, n_chunks);
     if (g_block_path) {          // a lane per BLOCK: zb_scan_blocks -> zb_entropy_blocks -> zb_resolve_blocks -> zb_patch_blocks
         u64 const nb = totals[1];
+        u32 const btake = chunk_bytes ? 3 : (take > 3 ? 3 : take);
+        u32 bctas = n_ctas; if (chunk_bytes) { u64 const need = (nb + 7 * btake - 1) / (7 * btake); if (bctas > need) bctas = (u32)need; if (bctas == 0) bctas = 1; }
+        u32 counter = 0;
         bdesc.resize(nb + 1); std::vector<ZbBlkExit> bexit(nb + 1); std::vector<u32> erep(3 * (nb + 1)); std::vector<u64> fend(n);
         simt::launch((n + 63) / 64, 64, [&] { zb_scan_blocks(src, segs.data(), n, place.data(), dict, status.data(), bdesc.data(), fend.data(), big.data()); });
         simt::launch(n < 128 ? (n + 3) / 4 : 32, 128, [&] { zb_scan_blocks_big(src, segs.data(), big.data(), place.data(), dict, status.data(), bdesc.data(), fend.data()); });
-        simt::launch(n_ctas, 7 * 32, [&] { zb_entropy_blocks<7>(src, bdesc.data(), (u32)nb, blocks.data(), seqs.data(), lits.data(), &counter, dict, status.data(), bexit.data(), take > 3 ? 3 : take); });
+        simt::launch(bctas, 7 * 32, [&] { zb_entropy_blocks<7>(src, bdesc.data(), (u32)nb, blocks.data(), seqs.data(), lits.data(), &counter, dict, status.data(), bexit.data(), btake); });
         simt::launch((n + 63) / 64, 64, [&] { zb_resolve_blocks(src, segs.data(), n, place.data(), info.data(), dst_sizes, blocks.data(), bdesc.data(), bexit.data(), fend.data(), dict, status.data(), out_sizes.data(), ck.data(), erep.data()); });
         if (nb) simt::launch((unsigned)((nb + 7) / 8), 256, [&] { zb_patch_blocks(blocks.data(), bdesc.data(), nb, seqs.data(), erep.data(), dict, status.data()); });
     }
-    else if (warps == 8) simt::launch(n_ctas, 8 * 32, [&] { zb_entropy_decode<8>(src, segs.data(), n, place.data(), dst_sizes, blocks.data(), seqs.data(), lits.data(), &counter, dict, status.data(), out_sizes.data(), ck.data(), take); });
-    else simt::launch(n_ctas, 7 * 32, [&] { zb_entropy_decode<7>(src, segs.data(), n, place.data(), dst_sizes, blocks.data(), seqs.data(), lits.data(), &counter, dict, status.data(), out_sizes.data(), ck.data(), take); });
-    simt::launch((n + ZB_TILE_WARPS - 1) / ZB_TILE_WARPS, ZB_TILE_WARPS * 32, [&] { zb_execute_tile(src, place.data(), status.data(), blocks.data(), seqs.data(), lits.data(), out, 0, n, dict); });
-    if (g_block_path == 2) {     // pointer-jumping execute stage (zb_chase_*): init, doubling rounds until nothing changes, gather
-        std::vector<u32> ptr(totals[0] + 16, 0xFFFFFFFFu); u32 changed = 0; int rounds = 0;
-        simt::launch(3, 256, [&] { zb_chase_init<u32>(src, place.data(), status.data(), blocks.data(), (const ZbBlkDesc*)bdesc.data(), seqs.data(), lits.data(), out, ptr.data(), 0, totals[1], dict); });
-        do { changed = 0; simt::launch(4, 256, [&] { zb_chase_round<u32>(ptr.data(), 0, totals[0], &changed); }); rounds++; } while (changed && rounds < 72);
-        simt::launch(4, 256, [&] { zb_chase_gather<u32>(ptr.data(), out, 0, totals[0], totals[0]); });
+    std::vector<u32> ptr(g_block_path == 2 ? totals[0] + 16 : 0);
+    u64 changed_bytes = 0, redone = 0;
+    std::vector<u64> sizes_aside(n);
+    std::vector<u8> copy(totals[0] + 64, 0);           // what the copy stream took, chunk by chunk
+    auto poison = [](u64 p) { return (u8)(1 + p % 251); };
+    for (u32 k = 0; k < n_chunks; k++) {
+        u32 const f0 = cut[k], f1 = cut[k + 1];
+        u64 const lo = n_chunks > 1 ? place[f0].dst_off : 0, hi = n_chunks > 1 ? place[f1].dst_off : totals[0];
+        u64 const blo = n_chunks > 1 ? place[f0].blk_off : 0, bhi = n_chunks > 1 ? place[f1].blk_off : totals[1];
+        ZbChunkShape sh; sh.warps = warps; sh.take = take; sh.ctas = n_ctas;
+        if (g_block_path) sh.warps = sh.take = sh.ctas = 0;
+        else if (chunk_bytes) sh = zb_chunk_shape(hi - lo, f1 - f0, n_ctas);
+        if (!g_block_path) {
+            u32 counter = f0;
+            if (sh.warps == 8) simt::launch(sh.ctas, 8 * 32, [&] { zb_entropy_decode<8>(src, segs.data(), f1, place.data(), dst_sizes, blocks.data(), seqs.data(), lits.data(), &counter, dict, status.data(), out_sizes.data(), ck.data(), sh.take); });
+            else simt::launch(sh.ctas, 7 * 32, [&] { zb_entropy_decode<7>(src, segs.data(), f1, place.data(), dst_sizes, blocks.data(), seqs.data(), lits.data(), &counter, dict, status.data(), out_sizes.data(), ck.data(), sh.take); });
+        }
+        if (g_block_path == 2) {     // pointer-jumping execute stage (zb_chase_*): init, doubling rounds until nothing changes, gather
+            if (hi > lo && bhi > blo) {
+                std::fill(ptr.begin() + lo, ptr.begin() + hi, 0xFFFFFFFFu); u32 changed = 0; int rounds = 0;
+                simt::launch(3, 256, [&] { zb_chase_init<u32>(src, place.data(), status.data(), blocks.data(), (const ZbBlkDesc*)bdesc.data(), seqs.data(), lits.data(), d_out, ptr.data(), blo, bhi, dict); });
+                do { changed = 0; simt::launch(4, 256, [&] { zb_chase_round<u32>(ptr.data(), lo, hi, &changed); }); rounds++; } while (changed && rounds < 72);
+                simt::launch(4, 256, [&] { zb_chase_gather<u32>(ptr.data(), d_out, lo, hi, totals[0]); });
+            }
+        }
+        else {
+            simt::launch((f1 - f0 + ZB_TILE_WARPS - 1) / ZB_TILE_WARPS, ZB_TILE_WARPS * 32, [&] { zb_execute_tile(src, place.data(), status.data(), blocks.data(), seqs.data(), lits.data(), d_out, f0, f1, dict); });
+            if (g_block_path && bhi > blo) {
+                std::vector<unsigned long long> w_done(n + 1, 0); std::vector<u32> w_pre(n + 1, 0), w_flag(totals[1] + 1, 0); u32 w_ticket = 0;
+                ZbWave w; w.done_pos = w_done.data(); w.pre_blk = w_pre.data(); w.blk_flag = w_flag.data(); w.ticket = &w_ticket;
+                simt::launch(3, ZB_BIG_NT, [&] { zb_execute_big(src, place.data(), status.data(), blocks.data(), (const ZbBlkDesc*)bdesc.data(), seqs.data(), lits.data(), d_out,
+                                                               blo, bhi, dict, (u64)ZB_TILE_CAP + 1, w); });
+            }
+            else if (!g_block_path) simt::launch((f1 - f0 + 7) / 8, 256, [&] { zb_execute(src, place.data(), status.data(), blocks.data(), seqs.data(), lits.data(), d_out, f0, f1, dict, (u64)ZB_TILE_CAP + 1); });
+        }
+        if (totals[4]) simt::launch((f1 - f0 + 127) / 128, 128, [&] { zb_verify_checksums(d_out, place.data(), out_sizes.data(), info.data(), ck.data(), f0, f1, status.data()); });
+        if (totals[4]) simt::launch(f1 - f0 < 8 ? f1 - f0 : 8, 256, [&] { zb_verify_checksums_big(d_out, place.data(), out_sizes.data(), info.data(), ck.data(), f0, f1, status.data()); });
+        // the copy of the chunk; the working buffer's bytes there are not read again
+        for (u64 p = lo; p < hi; p++) { copy[p] = d_out[p]; d_out[p] ^= poison(p); }
+        for (u32 f = f0; f < f1; f++) { sizes_aside[f] = out_sizes[f]; out_sizes[f] = ~0ull; }
+        if (plan && k < 33) { u64* c = plan + 3 + 5 * k; c[0] = f0; c[1] = sh.warps; c[2] = sh.take; c[3] = sh.ctas; c[4] = hi - lo; }
     }
-    else if (g_block_path) {
-        std::vector<unsigned long long> w_done(n + 1, 0); std::vector<u32> w_pre(n + 1, 0), w_flag(totals[1] + 1, 0); u32 w_ticket = 0;
-        ZbWave w; w.done_pos = w_done.data(); w.pre_blk = w_pre.data(); w.blk_flag = w_flag.data(); w.ticket = &w_ticket;
-        simt::launch(3, ZB_BIG_NT, [&] { zb_execute_big(src, place.data(), status.data(), blocks.data(), (const ZbBlkDesc*)bdesc.data(), seqs.data(), lits.data(), out,
-                                                       0, totals[1], dict, (u64)ZB_TILE_CAP + 1, w); });
-    }
-    else simt::launch((n + 7) / 8, 256, [&] { zb_execute(src, place.data(), status.data(), blocks.data(), seqs.data(), lits.data(), out, 0, n, dict, (u64)ZB_TILE_CAP + 1); });
-    if (totals[4]) simt::launch((n + 127) / 128, 128, [&] { zb_verify_checksums(out, place.data(), out_sizes.data(), info.data(), ck.data(), 0, n, status.data()); });
-    if (totals[4]) simt::launch(n < 8 ? n : 8, 256, [&] { zb_verify_checksums_big(out, place.data(), out_sizes.data(), info.data(), ck.data(), 0, n, status.data()); });
+    for (u64 p = 0; p < totals[0]; p++) changed_bytes += d_out[p] != (u8)(copy[p] ^ poison(p));
+    for (u32 f = 0; f < n; f++) { redone += out_sizes[f] != ~0ull; out_sizes[f] = sizes_aside[f]; }
+    memcpy(out, copy.data(), totals[0]);
+    if (plan) { plan[0] = n_chunks; plan[1] = changed_bytes; plan[2] = redone; }
     std::vector<ZbSegment> out_segs(n); u32 first_error = 0xFFFFFFFFu;
     simt::launch((n + 255) / 256, 256, [&] { zb_finish(place.data(), out_sizes.data(), status.data(), n, out_segs.data(), &first_error); });
     for (u32 i = 0; i < n; i++) { out_off[i] = out_segs[i].offset; out_len[i] = out_segs[i].length; status_out[i] = status[i]; }
@@ -382,7 +432,8 @@ def build_decode_sim():
     L = C.CDLL(DSIM_LIB)
     L.t_decompress_batch.restype = C.c_longlong
     L.t_decompress_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32,
-                                     C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+                                     C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                     C.c_uint64, C.c_void_p]
     L.t_scan_totals.restype = None
     L.t_scan_totals.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
     return L

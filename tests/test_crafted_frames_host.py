@@ -132,7 +132,7 @@ def _batch(sim, frames, sizes, dct, gaps, warps, take, n_ctas=2):
     oo = (C.c_uint64 * n)(); ol = (C.c_uint64 * n)(); st = (C.c_uint32 * n)()
     want = (C.c_uint64 * n)(*sizes)
     tot = sim.t_decompress_batch(C.addressof(src), off.ctypes.data, ln.ctypes.data, n, (C.addressof(dbuf) + PAD) if dct else None, len(dct),
-                                 n_ctas, warps, take, C.addressof(out), cap, C.addressof(oo), C.addressof(ol), C.addressof(st), C.addressof(want))
+                                 n_ctas, warps, take, C.addressof(out), cap, C.addressof(oo), C.addressof(ol), C.addressof(st), C.addressof(want), 0, None)
     if tot < 0:
         return None, None
     return [bytes(out[oo[i]:oo[i] + ol[i]]) for i in range(n)], list(st)

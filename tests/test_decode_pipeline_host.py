@@ -36,7 +36,7 @@ def ref():
 
 
 def decompress(sim, frames, sizes, dct=b"", n_ctas=1, warps=8, take=32, exact_sizes=False):
-    """(outputs, statuses) of a batch of frames through the kernels."""
+    """(outputs, statuses) of a batch of frames through the kernels, in one chunk."""
     blob = bytes(PAD) + b"".join(frames) + bytes(PAD)
     off = (np.cumsum([0] + [len(f) for f in frames[:-1]]) + PAD).astype(np.uint64)
     ln = np.array([len(f) for f in frames], dtype=np.uint64)
@@ -49,7 +49,7 @@ def decompress(sim, frames, sizes, dct=b"", n_ctas=1, warps=8, take=32, exact_si
     want = (C.c_uint64 * n)(*sizes)                                # decompressed_sizes of the batch call, when given
     tot = sim.t_decompress_batch(C.addressof(src), off.ctypes.data, ln.ctypes.data, n, (C.addressof(dbuf) + PAD) if dct else None, len(dct),
                                  n_ctas, warps, take, C.addressof(out), cap, C.addressof(oo), C.addressof(ol), C.addressof(st),
-                                 C.addressof(want) if exact_sizes else None)
+                                 C.addressof(want) if exact_sizes else None, 0, None)
     assert tot >= 0
     return [bytes(out[oo[i]:oo[i] + ol[i]]) for i in range(n)], list(st)
 

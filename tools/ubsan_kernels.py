@@ -16,7 +16,7 @@ ref=RefZstd()
 Lc=C.CDLL('/tmp/libzs_ubsan.so'); Lc.t_compress_batch.restype=C.c_longlong
 Lc.t_compress_batch.argtypes=[C.c_void_p,C.c_void_p,C.c_void_p,C.c_uint32,C.c_uint32,C.c_uint32,C.c_uint32,C.c_void_p,C.c_uint64,C.c_void_p,C.c_void_p,C.c_uint32,C.c_void_p,C.c_uint32,C.c_int,C.c_uint32]
 Ld=C.CDLL('/tmp/libzd_ubsan.so'); Ld.t_decompress_batch.restype=C.c_longlong
-Ld.t_decompress_batch.argtypes=[C.c_void_p,C.c_void_p,C.c_void_p,C.c_uint32,C.c_void_p,C.c_uint32,C.c_uint32,C.c_uint32,C.c_uint32,C.c_void_p,C.c_uint64,C.c_void_p,C.c_void_p,C.c_void_p,C.c_void_p]
+Ld.t_decompress_batch.argtypes=[C.c_void_p,C.c_void_p,C.c_void_p,C.c_uint32,C.c_void_p,C.c_uint32,C.c_uint32,C.c_uint32,C.c_uint32,C.c_void_p,C.c_uint64,C.c_void_p,C.c_void_p,C.c_void_p,C.c_void_p,C.c_uint64,C.c_void_p]
 text=corpus.text_corpus(1<<20)
 segs=[b"foo"*12,b"",bytes(text[:4096]),bytes(text[5000:6500]),bytes(text[10000:10000+131072]),bytes(9000),np.random.default_rng(1).integers(0,256,7000).astype(np.uint8).tobytes()]
 for dual in (False,True):

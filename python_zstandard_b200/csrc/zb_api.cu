@@ -385,9 +385,9 @@ int zb200_ddict_create(zb200_ctx* ctx, const void* dict, size_t size, zb200_ddic
     v.rep[0] = h->rep[0]; v.rep[1] = h->rep[1]; v.rep[2] = h->rep[2];
     free(h);
     // compression view (built now, it is one tiny launch)
-    d->c_D = v.content_size < 32768u ? v.content_size : 32768u;
-    d->c_tail = v.content + (v.content_size - d->c_D);
-    if (d->c_D >= 8 && cudaMalloc((void**)&d->d_ctable, 16384 * sizeof(u16)) == cudaSuccess) {
+    ZbDictView const cv = zb_dict_view(v.content, v.content_size);
+    d->c_tail = cv.tail; d->c_D = cv.D;
+    if (d->c_D && cudaMalloc((void**)&d->d_ctable, 16384 * sizeof(u16)) == cudaSuccess) {
         zb_launch_dict_table(d->c_tail, d->c_D, d->d_ctable, ctx->stream);
         if (v.has_entropy && cudaMalloc(&d->d_cct, 3 * (size_t)zb_encode_ctable_bytes()) == cudaSuccess)
             zb_launch_dict_ctables(d->d_digest, d->d_cct, ctx->stream);
@@ -504,11 +504,9 @@ static int run_decompress(zb200_ctx* ctx, const u8* d_src, const ZbSegment* d_se
         else if (chase_path && ctx->chase.ensure(zb_chase_bytes(totals[0])) != cudaSuccess) { cudaGetLastError(); chase_path = false; }
         { KSpan s(ctx, ZB200_K_SCAN);
           zb_launch_scan_blocks(d_src, d_segs, nf, ctx->place.as<ZbFramePlace>(), dd, ctx->status.as<u32>(), ctx->bdesc.p, ctx->fend.as<u64>(), ctx->biglist.as<u32>(), ctx->stream); }
-        u32 const take = 3, EW = 7;
-        u32 cc = ctas; { u64 const need = (nb + EW * take - 1) / (EW * take); if (cc > need) cc = (u32)need; if (cc == 0) cc = 1; }
         { KSpan s(ctx, ZB200_K_ENTROPY);
-          zb_launch_entropy_blocks(d_src, ctx->bdesc.p, (u32)nb, ctx->blocks.as<ZbBlock>(), ctx->seqs.as<ZbSeq>(), ctx->lits.as<u8>(), cc, d_counter, dd,
-                                   ctx->status.as<u32>(), ctx->bexit.p, take, ctx->stream); }
+          zb_launch_entropy_blocks(d_src, ctx->bdesc.p, (u32)nb, ctx->blocks.as<ZbBlock>(), ctx->seqs.as<ZbSeq>(), ctx->lits.as<u8>(),
+                                   zb_entropy_blocks_ctas(nb, ctas), d_counter, dd, ctx->status.as<u32>(), ctx->bexit.p, ZB_BLOCKS_TAKE, ctx->stream); }
         { KSpan s(ctx, ZB200_K_PLACE);
           zb_launch_resolve_blocks(d_src, d_segs, nf, ctx->place.as<ZbFramePlace>(), ctx->info.as<ZbFrameInfo>(), exact_sizes ? d_dst_sizes : nullptr,
                                    ctx->blocks.as<ZbBlock>(), ctx->bdesc.p, ctx->bexit.p, ctx->fend.as<u64>(), nb, ctx->seqs.as<ZbSeq>(), dd,
@@ -855,7 +853,7 @@ static int compress_common(zb200_ctx* ctx, const void* src_base, const zb200_seg
     jobs.reserve(n);
     u32 const max_block = zb_cut_blocks(hsegs.data(), n, block_max, jobs, sinfo);
     size_t const nj = jobs.size();
-    u64 const slot_bytes = ((u64)max_block + (max_block >> 7) + 64 + 15) & ~15ull;
+    u64 const slot_bytes = zb_slot_bytes(max_block);
     // Blocks of 8 KiB and more (no dictionary, level-3 class) take the round-2 kernel: one CTA per SM with the block resident in
     // shared memory.  Small blocks, dictionaries and the level >= 4 mode stay on the CTA-per-block kernel (6 CTAs per SM).
     static int const force_v1 = getenv("ZB200_ENCODER_V1") ? atoi(getenv("ZB200_ENCODER_V1")) : 0;
@@ -984,12 +982,6 @@ int zb200_compress_batch_ptrs(zb200_ctx* ctx, const void* const* srcs, const siz
 // (zb_chain_index), every block through the prefix mode of zb_compress_blocks, the frames laid out by the batch kernels with
 // window_log 31 (single segment: the window is the content size, so offsets may reach the whole prefix, RFC 8878 section 3.1.1.1.2).
 namespace {
-u32 chain_log(u64 len)          // a chunk's index: 2^log slots for the two keys of its sampled positions at a load of at most 1/2, >= 16 slots
-{
-    u64 const npos = len >= 8 ? (len - 8) / 4 + 1 : 0;
-    u32 L = 4; while ((1ull << L) < 4 * npos) L++;
-    return L;
-}
 struct HostChainSeg { u64 start; const u32* tab; const u32* prev_tab; u32 len, prev_len, log, prev_log; };    // == ZeChainSeg
 }
 
@@ -1023,8 +1015,8 @@ int zb200_compress_chain(zb200_ctx* ctx, const void* const* srcs, const size_t* 
         size_t fr = 0, tot = 0; cudaMemGetInfo(&fr, &tot);
         budget = env && *env ? strtoull(env, nullptr, 10) : (u64)fr / 10 * 6;
     }
-    auto cost = [&](size_t j) { return (u64)sizes[j] + (4ull << chain_log(sizes[j])) + sizes[j] + (sizes[j] >> 7) + 4096 + 200 * (sizes[j] / ZB_BLOCK_MAX + 1); };
-    u64 const slot_bytes = ((u64)ZB_BLOCK_MAX + (ZB_BLOCK_MAX >> 7) + 64 + 15) & ~15ull;
+    auto cost = [&](size_t j) { return (u64)sizes[j] + (4ull << zb_chain_log(sizes[j])) + sizes[j] + (sizes[j] >> 7) + 4096 + 200 * (sizes[j] / ZB_BLOCK_MAX + 1); };
+    u64 const slot_bytes = zb_slot_bytes(ZB_BLOCK_MAX);
     u32 const ctas_max = (u32)ctx->sm_count * (227u * 1024u / zb_encode_smem_bytes());
     size_t k = 1;
     while (k < n) {
@@ -1036,31 +1028,15 @@ int zb200_compress_chain(zb200_ctx* ctx, const void* const* srcs, const size_t* 
         u8* stage = (u8*)pinned_get(ctx, total + 128);
         if (!stage) return fail(ctx, "pinned staging allocation", cudaErrorMemoryAllocation);
         memset(stage, 0, 64); memset(stage + 64 + total, 0, 64);
-        std::vector<HostChainSeg> cs(m); std::vector<u64> tab_off(m + 1, 0), pos_off(m + 1, 0);
-        {
-            u64 pos = 64;
-            for (size_t i = 0; i < m; i++) {
-                size_t const j = k - 1 + i;
-                if (sizes[j]) memcpy(stage + pos, srcs[j], sizes[j]);
-                cs[i].start = pos; cs[i].len = (u32)sizes[j]; cs[i].log = chain_log(sizes[j]);
-                cs[i].prev_len = i ? (u32)sizes[j - 1] : 0; cs[i].prev_log = i ? cs[i - 1].log : 0;
-                tab_off[i + 1] = tab_off[i] + (1ull << cs[i].log);
-                pos_off[i + 1] = pos_off[i] + (sizes[j] >= 8 ? (sizes[j] - 8) / 4 + 1 : 0);
-                pos += sizes[j];
-            }
+        // the chunks in the staging buffer; chunks 1..m-1 are the frames' segments
+        std::vector<zb200_segment> rsegs(m);
+        for (size_t i = 0, pos = 64; i < m; pos += sizes[k - 1 + i], i++) {
+            if (sizes[k - 1 + i]) memcpy(stage + pos, srcs[k - 1 + i], sizes[k - 1 + i]);
+            rsegs[i].offset = pos; rsegs[i].length = sizes[k - 1 + i];
         }
-        // block jobs of the chunks after the prefix; job.seg indexes the run's descriptors, the layout tables its frames
-        std::vector<HostJob> jobs; std::vector<HostSegInfo> sinfo(m - 1); std::vector<zb200_segment> lsegs(m - 1);
-        for (size_t i = 1; i < m; i++) {
-            u64 const len = cs[i].len;
-            lsegs[i - 1].offset = cs[i].start; lsegs[i - 1].length = len;
-            sinfo[i - 1].first_job = jobs.size(); sinfo[i - 1].n_jobs = 0; sinfo[i - 1].pad = 0;
-            for (u64 pos = 0; pos < len;) {
-                u32 const sz = (u32)(len - pos < ZB_BLOCK_MAX ? len - pos : ZB_BLOCK_MAX);
-                HostJob j; j.src_pos = cs[i].start + pos; j.size = sz; j.seg = (u32)i; j.first = pos == 0; j.last = pos + sz == len;
-                jobs.push_back(j); sinfo[i - 1].n_jobs++; pos += sz;
-            }
-        }
+        std::vector<HostChainSeg> cs(m); std::vector<u64> tab_off(m + 1), pos_off(m + 1);
+        std::vector<HostJob> jobs; std::vector<HostSegInfo> sinfo(m - 1);
+        zb_chain_plan(rsegs.data(), m, cs.data(), tab_off.data(), pos_off.data(), jobs, sinfo);
         size_t const nj = jobs.size(), nf = m - 1;
         u32 ctas = ctas_max; if (ctas > nj) ctas = (u32)nj; if (ctas == 0) ctas = 1;
         cudaError_t e = ctx->src.ensure(total + 128);
@@ -1084,7 +1060,7 @@ int zb200_compress_chain(zb200_ctx* ctx, const void* const* srcs, const size_t* 
         if (e == cudaSuccess) e = cudaMemsetAsync(d_tab, 0xFF, tab_off[m] * 4, ctx->stream);
         if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->chain_seg.p, cs.data(), m * sizeof(HostChainSeg), cudaMemcpyHostToDevice, ctx->stream);
         if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->chain_pos.p, pos_off.data(), (m + 1) * sizeof(u64), cudaMemcpyHostToDevice, ctx->stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->segs.p, lsegs.data(), nf * sizeof(ZbSegment), cudaMemcpyHostToDevice, ctx->stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->segs.p, rsegs.data() + 1, nf * sizeof(ZbSegment), cudaMemcpyHostToDevice, ctx->stream);
         if (e == cudaSuccess && nj) e = cudaMemcpyAsync(ctx->jobs.p, jobs.data(), nj * sizeof(HostJob), cudaMemcpyHostToDevice, ctx->stream);
         if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->seginfo.p, sinfo.data(), nf * sizeof(HostSegInfo), cudaMemcpyHostToDevice, ctx->stream);
         if (e == cudaSuccess) e = cudaMemsetAsync(d_counter, 0, 64, ctx->stream);

@@ -43,6 +43,18 @@ enum : u32 {
 
 struct ZbSegment { u64 offset, length; };       // == BufferSegment, c-ext/python-zstandard.h:307-313
 
+// ---- kernel launches.  The launchers launch through ZB_LAUNCH, and the kernels name their dynamic shared memory with
+// ZB_DYN_SMEM (zb_decode.cu, zb_encode.cu), so that the CPU build of these sources (ZB_SIMT_EMULATION, tests/simt.h) runs
+// the very launches the device runs.  Pass a template kernel parenthesised: (k<a, b>).  On the device every launch with
+// dynamic shared memory first raises the kernel's limit to it (per device: cheap, so set on every launch).
+#ifdef ZB_SIMT_EMULATION
+#define ZB_LAUNCH(kernel, grid, block, smem, stream, ...) simt::launch((grid), (block), [&] { kernel(__VA_ARGS__); })
+#else
+#define ZB_LAUNCH(kernel, grid, block, smem, stream, ...) do { \
+        if (smem) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(smem)); \
+        kernel<<<(grid), (block), (smem), (stream)>>>(__VA_ARGS__); } while (0)
+#endif
+
 // Block_Maximum_Size = min(window, 128 KiB) (ZSTD_getBlockSize, zstd/zstd.c:27478): a window_log below 17 cuts blocks of
 // 2^window_log bytes, and with them the reach of every match; 0 = the default window
 static inline u32 zb_block_max(u32 window_log) { return window_log && window_log < 17 ? (1u << window_log) : ZB_BLOCK_MAX; }
@@ -67,6 +79,59 @@ static inline u32 zb_cut_blocks(const Seg* segs, size_t n, u32 block_max, JobVec
         }
     }
     return max_block;
+}
+
+// The output slot of one block job: a block of up to max_block bytes compresses to at most this many (raw block fallback,
+// headers, the entropy coders' slack), rounded up to 16 bytes.
+static inline u64 zb_slot_bytes(u32 max_block) { return ((u64)max_block + (max_block >> 7) + 64 + 15) & ~15ull; }
+
+// The compression view of a dictionary: the last <= 32 KiB of its content act as history in front of every frame
+// (zb200_ddict_create).  Fewer than 8 bytes are not used: D = 0.
+struct ZbDictView { const u8* tail; u32 D; };
+static inline ZbDictView zb_dict_view(const u8* content, u32 content_size)
+{
+    u32 const D = content_size < 32768u ? content_size : 32768u;
+    ZbDictView v; v.tail = content + (content_size - D); v.D = D >= 8 ? D : 0;
+    return v;
+}
+
+// Content-dictionary chains (zb200_compress_chain).  A chunk's index samples every ZE_CHAIN_STEP-th position with 8 bytes
+// behind it and holds 2^log slots for the two keys of each, at a load of at most 1/2 and at least 16 slots.
+#define ZE_CHAIN_STEP 4u                // backward extension finds the true match starts
+static inline u64 zb_chain_positions(u64 len) { return len >= 8 ? (len - 8) / ZE_CHAIN_STEP + 1 : 0; }
+static inline u32 zb_chain_log(u64 len)
+{
+    u64 const npos = zb_chain_positions(len);
+    u32 L = 4; while ((1ull << L) < 4 * npos) L++;
+    return L;
+}
+// The plan of one run of a chain: chunks[0] is the prefix of chunks[1] only, chunks 1..m-1 become frames, and chunks[1..m)
+// are the frames' segments.  Fills each chunk's index descriptor except its device pointers (tab, prev_tab), the offsets of
+// the chunks' indexes in the run's slot array (tab_off, m + 1 entries) and of their sampled positions (pos_off, m + 1), and
+// the block jobs of the frames (ZB_BLOCK_MAX blocks, job.seg = the chunk's descriptor) with their layout info (m - 1 entries).
+template <class Seg, class Desc, class JobVec, class InfoVec>
+static inline void zb_chain_plan(const Seg* chunks, size_t m, Desc* cs, u64* tab_off, u64* pos_off, JobVec& jobs, InfoVec& info)
+{
+    tab_off[0] = pos_off[0] = 0;
+    for (size_t i = 0; i < m; i++) {
+        u64 const len = chunks[i].length;
+        cs[i].start = chunks[i].offset; cs[i].len = (u32)len; cs[i].log = zb_chain_log(len);
+        cs[i].prev_len = i ? cs[i - 1].len : 0; cs[i].prev_log = i ? cs[i - 1].log : 0;
+        tab_off[i + 1] = tab_off[i] + (1ull << cs[i].log);
+        pos_off[i + 1] = pos_off[i] + zb_chain_positions(len);
+    }
+    zb_cut_blocks(chunks + 1, m - 1, ZB_BLOCK_MAX, jobs, info);
+    for (auto& j : jobs) j.seg++;
+}
+
+// The CTA count of the lane-per-block entropy launch (zb_entropy_blocks: 7 warps, ZB_BLOCKS_TAKE blocks per lane): one CTA
+// per SM, fewer when the blocks do not fill them.
+#define ZB_BLOCKS_TAKE 3u
+static inline u32 zb_entropy_blocks_ctas(u64 n_blocks, u32 sm_count)
+{
+    u64 const need = (n_blocks + 7 * ZB_BLOCKS_TAKE - 1) / (7 * ZB_BLOCKS_TAKE);
+    u32 const c = sm_count < need ? sm_count : (u32)need;
+    return c ? c : 1;
 }
 
 // The output chunks of a batch decode (run_decompress, zb_api.cu): a call whose output is copied back to the host is cut

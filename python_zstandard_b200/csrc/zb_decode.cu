@@ -13,6 +13,16 @@
 //   K4 zb_execute         one WARP per frame : the LZ copy-execute, lane per sequence with a
 //                          frontier test for match dependencies, coalesced copies for long runs.
 #include "zb_common.cuh"
+// A kernel's dynamic shared memory.  The CPU build of these sources (ZB_SIMT_EMULATION, tests/simt.h) runs one CTA at a time
+// and points every kernel at simt.h's static buffer.  Defined with the kernels rather than in zb_common.cuh, and word for word
+// the same in zb_decode.cu and zb_encode.cu: host builds of the kernel text that define ZB_SIMT_EMULATION after that header,
+// or that rewrite this declaration line, get the CPU form too.
+#ifdef ZB_SIMT_EMULATION
+#define ZB_DYN_SMEM(name) u8* const name = simt_dyn_smem;
+#else
+#define ZB_DYN_SMEM(name) extern __shared__ __align__(16) u8 name[];
+#endif
+
 #ifdef ZB_DEBUG_BLOCKS
 #include <cstdio>
 #endif
@@ -948,7 +958,7 @@ zb_execute_tile(const u8* __restrict__ src, const ZbFramePlace* __restrict__ pla
                 const ZbBlock* __restrict__ blocks, const ZbSeq* __restrict__ seqs, const u8* __restrict__ lits,
                 u8* __restrict__ dst, u32 first, u32 n_frames, ZbDictDev dict)
 {
-    extern __shared__ __align__(16) u8 zb_tile[];
+    ZB_DYN_SMEM(zb_tile);
     u32 const lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     u32 const f = first + blockIdx.x * ZB_TILE_WARPS + warp;                    // frames [first, n_frames)
     if (f >= n_frames) return;
@@ -1160,7 +1170,7 @@ zb_execute_big(const u8* __restrict__ src, const ZbFramePlace* __restrict__ plac
                const ZbBlock* __restrict__ blocks, const ZbBlkDesc* __restrict__ bdesc, const ZbSeq* __restrict__ seqs,
                const u8* __restrict__ lits, u8* dst, u64 blk_first, u64 blk_last, ZbDictDev dict, u64 min_cap, ZbWave wave)
 {
-    extern __shared__ __align__(16) u8 zb_big[];
+    ZB_DYN_SMEM(zb_big);
     __shared__ u32 s_ticket;
     u32 const tid = threadIdx.x, lane = tid & 31;
     const u8* const dict_end = dict.content + dict.content_size;
@@ -1711,37 +1721,36 @@ __global__ void zb_digest_dict(const u8* __restrict__ dict, u32 n, ZbDictDigest*
 // ===========================================================================
 extern "C" {
 
-void zb_launch_default_tables(cudaStream_t st) { zb_build_default_tables<<<1, 32, 0, st>>>(); }
+void zb_launch_default_tables(cudaStream_t st) { ZB_LAUNCH(zb_build_default_tables, 1, 32, 0, st); }
 
 void zb_launch_scan(const u8* src, const ZbSegment* segs, u32 n, ZbFrameInfo* info, u64 window_limit, u32* big_list, cudaStream_t st)
 {
     // big_list: n + 1 words; [0] = number of frames left to zb_scan_frames_big
     cudaMemsetAsync(big_list, 0, sizeof(u32), st);
-    zb_scan_frames<<<(n + 127) / 128, 128, 0, st>>>(src, segs, n, info, window_limit, big_list);
-    zb_scan_frames_big<<<n < 128 ? (n + 3) / 4 : 32, 128, 0, st>>>(src, segs, big_list, info);
+    ZB_LAUNCH(zb_scan_frames, (n + 127) / 128, 128, 0, st, src, segs, n, info, window_limit, big_list);
+    ZB_LAUNCH(zb_scan_frames_big, n < 128 ? (n + 3) / 4 : 32, 128, 0, st, src, segs, big_list, info);
 }
 
 void zb_launch_scan_blocks(const u8* src, const ZbSegment* segs, u32 n, const ZbFramePlace* place, ZbDictDev dict, u32* status,
                            void* bdesc, u64* frame_end, const u32* big_list, cudaStream_t st)
 {
-    zb_scan_blocks<<<(n + 63) / 64, 64, 0, st>>>(src, segs, n, place, dict, status, (ZbBlkDesc*)bdesc, frame_end, big_list);
-    zb_scan_blocks_big<<<n < 128 ? (n + 3) / 4 : 32, 128, 0, st>>>(src, segs, big_list, place, dict, status, (ZbBlkDesc*)bdesc, frame_end);
+    ZB_LAUNCH(zb_scan_blocks, (n + 63) / 64, 64, 0, st, src, segs, n, place, dict, status, (ZbBlkDesc*)bdesc, frame_end, big_list);
+    ZB_LAUNCH(zb_scan_blocks_big, n < 128 ? (n + 3) / 4 : 32, 128, 0, st, src, segs, big_list, place, dict, status, (ZbBlkDesc*)bdesc, frame_end);
 }
 void zb_launch_entropy_blocks(const u8* src, const void* bdesc, u32 n_blocks, ZbBlock* blocks, ZbSeq* seqs, u8* lits, u32 n_ctas, u32* work_counter,
                               ZbDictDev dict, u32* status, void* bexit, u32 take, cudaStream_t st)
 {
-    cudaFuncSetAttribute(zb_entropy_blocks<7>, cudaFuncAttributeMaxDynamicSharedMemorySize, ZB_ENT_SMEM(7));
-    zb_entropy_blocks<7><<<n_ctas, 7 * 32, ZB_ENT_SMEM(7), st>>>(src, (const ZbBlkDesc*)bdesc, n_blocks, blocks, seqs, lits, work_counter, dict, status,
-                                                                (ZbBlkExit*)bexit, take);
+    ZB_LAUNCH(zb_entropy_blocks<7>, n_ctas, 7 * 32, ZB_ENT_SMEM(7), st, src, (const ZbBlkDesc*)bdesc, n_blocks, blocks, seqs, lits, work_counter, dict,
+              status, (ZbBlkExit*)bexit, take);
 }
 void zb_launch_resolve_blocks(const u8* src, const ZbSegment* segs, u32 n, const ZbFramePlace* place, const ZbFrameInfo* info, const u64* dst_sizes,
                               ZbBlock* blocks, const void* bdesc, const void* bexit, const u64* frame_end, u64 n_blocks, ZbSeq* seqs, ZbDictDev dict,
                               u32* status, u64* out_sizes, u32* ck_expect, u32* entry_rep, cudaStream_t st, int chain)
 {
-    zb_resolve_blocks<<<(n + 63) / 64, 64, 0, st>>>(src, segs, n, place, info, dst_sizes, blocks, (const ZbBlkDesc*)bdesc, (const ZbBlkExit*)bexit,
-                                                   frame_end, dict, status, out_sizes, ck_expect, entry_rep);
-    if (n_blocks) zb_patch_blocks<<<(unsigned)((n_blocks + 7) / 8), 256, 0, st>>>(blocks, (const ZbBlkDesc*)bdesc, n_blocks, seqs, entry_rep, dict, status,
-                                                                                    chain ? place : nullptr);
+    ZB_LAUNCH(zb_resolve_blocks, (n + 63) / 64, 64, 0, st, src, segs, n, place, info, dst_sizes, blocks, (const ZbBlkDesc*)bdesc, (const ZbBlkExit*)bexit,
+              frame_end, dict, status, out_sizes, ck_expect, entry_rep);
+    if (n_blocks) ZB_LAUNCH(zb_patch_blocks, (unsigned)((n_blocks + 7) / 8), 256, 0, st, blocks, (const ZbBlkDesc*)bdesc, n_blocks, seqs, entry_rep, dict,
+                            status, chain ? place : nullptr);
 }
 size_t zb_blkdesc_bytes() { return sizeof(ZbBlkDesc); }
 size_t zb_blkexit_bytes() { return sizeof(ZbBlkExit); }
@@ -1750,8 +1759,8 @@ void zb_launch_place(const ZbFrameInfo* info, const u64* dst_sizes, u32 n, ZbFra
                      u32* status, u64* partial, cudaStream_t st)
 {
     u32 const ctas = (n + ZB_PLACE_CTA - 1) / ZB_PLACE_CTA;
-    zb_place_reduce<<<ctas, ZB_PLACE_CTA, 0, st>>>(info, dst_sizes, n, partial);
-    zb_place_scan<<<ctas, ZB_PLACE_CTA, 0, st>>>(info, dst_sizes, n, partial, place, totals, status);
+    ZB_LAUNCH(zb_place_reduce, ctas, ZB_PLACE_CTA, 0, st, info, dst_sizes, n, partial);
+    ZB_LAUNCH(zb_place_scan, ctas, ZB_PLACE_CTA, 0, st, info, dst_sizes, n, partial, place, totals, status);
 }
 
 void zb_launch_entropy(const u8* src, const ZbSegment* segs, u32 n, const ZbFramePlace* place, const u64* dst_sizes,
@@ -1759,15 +1768,10 @@ void zb_launch_entropy(const u8* src, const ZbSegment* segs, u32 n, const ZbFram
                        ZbDictDev dict, u32* status, u64* out_sizes, u32* ck_expect, u32 take, u32 warps, cudaStream_t st)
 {
     // persistent grid: one CTA of `warps` (7 or 8) warps per SM, each warp with its own shared-memory table pool
-    if (warps == 8) {
-        cudaFuncSetAttribute(zb_entropy_decode<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, ZB_ENT_SMEM(8));      // per device: cheap, so set on every launch
-        zb_entropy_decode<8><<<n_ctas, 8 * 32, ZB_ENT_SMEM(8), st>>>(src, segs, n, place, dst_sizes, blocks, seqs, lits,
-                                                                    work_counter, dict, status, out_sizes, ck_expect, take);
-    } else {
-        cudaFuncSetAttribute(zb_entropy_decode<7>, cudaFuncAttributeMaxDynamicSharedMemorySize, ZB_ENT_SMEM(7));
-        zb_entropy_decode<7><<<n_ctas, 7 * 32, ZB_ENT_SMEM(7), st>>>(src, segs, n, place, dst_sizes, blocks, seqs, lits,
-                                                                    work_counter, dict, status, out_sizes, ck_expect, take);
-    }
+    if (warps == 8) ZB_LAUNCH(zb_entropy_decode<8>, n_ctas, 8 * 32, ZB_ENT_SMEM(8), st, src, segs, n, place, dst_sizes, blocks, seqs, lits,
+                              work_counter, dict, status, out_sizes, ck_expect, take);
+    else ZB_LAUNCH(zb_entropy_decode<7>, n_ctas, 7 * 32, ZB_ENT_SMEM(7), st, src, segs, n, place, dst_sizes, blocks, seqs, lits,
+                   work_counter, dict, status, out_sizes, ck_expect, take);
 }
 
 // the pointer-jumping execute stage over the blocks [blk_first, blk_last) whose output is dst[lo, hi).  ptr_mem: (n_total + 16)
@@ -1784,21 +1788,21 @@ static int zb_chase_run(const u8* src, const ZbFramePlace* place, const u32* sta
     if (hi <= lo || blk_last <= blk_first) return 0;
     if (cudaMemsetAsync(ptr + lo, 0xFF, (hi - lo) * sizeof(P), st) != cudaSuccess) return -1;      // frames that failed stay "done, no source"
     u64 const nb = blk_last - blk_first;
-    if (chain) zb_chase_prefix<P><<<n_ctas * 4, 256, 0, st>>>(place, ptr);
-    zb_chase_init<P><<<(unsigned)(nb < n_ctas * 8ull ? nb : n_ctas * 8ull), 256, 0, st>>>(src, place, status, blocks, (const ZbBlkDesc*)bdesc, seqs, lits,
-                                                                                         dst, ptr, blk_first, blk_last, dict, chain);
+    if (chain) ZB_LAUNCH(zb_chase_prefix<P>, n_ctas * 4, 256, 0, st, place, ptr);
+    ZB_LAUNCH(zb_chase_init<P>, (unsigned)(nb < n_ctas * 8ull ? nb : n_ctas * 8ull), 256, 0, st, src, place, status, blocks, (const ZbBlkDesc*)bdesc, seqs,
+              lits, dst, ptr, blk_first, blk_last, dict, chain);
     u64 const want = (hi - lo + 255) / 256;
     unsigned const grid = (unsigned)(want < n_ctas * 16ull ? want : n_ctas * 16ull);
     int rounds = 0;
     for (; rounds < 72; rounds++) {
         u32 h = 0;
         if (cudaMemsetAsync(d_changed, 0, sizeof(u32), st) != cudaSuccess) return -1;
-        zb_chase_round<P><<<grid, 256, 0, st>>>(ptr, lo, hi, d_changed);
+        ZB_LAUNCH(zb_chase_round<P>, grid, 256, 0, st, ptr, lo, hi, d_changed);
         if (cudaMemcpyAsync(&h, d_changed, sizeof(u32), cudaMemcpyDeviceToHost, st) != cudaSuccess) return -1;
         if (cudaStreamSynchronize(st) != cudaSuccess) return -1;
         if (!h) { rounds++; break; }
     }
-    zb_chase_gather<P><<<grid, 256, 0, st>>>(ptr, dst, lo, hi, n_total);
+    ZB_LAUNCH(zb_chase_gather<P>, grid, 256, 0, st, ptr, dst, lo, hi, n_total);
     return rounds;
 }
 }
@@ -1819,11 +1823,9 @@ void zb_launch_execute_big(const u8* src, const ZbFramePlace* place, const u32* 
 {
     // the block-parallel path: few frames of many blocks.  Small frames as always; the blocks of the others are taken in
     // order by a persistent grid (16 warps and 219 KB of shared memory per CTA, one CTA per SM)
-    cudaFuncSetAttribute(zb_execute_tile, cudaFuncAttributeMaxDynamicSharedMemorySize, ZB_TILE_SMEM);
-    cudaFuncSetAttribute(zb_execute_big, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ZB_BIG_SMEM);
     u32 const n = end - first;
-    zb_execute_tile<<<(n + ZB_TILE_WARPS - 1) / ZB_TILE_WARPS, ZB_TILE_WARPS * 32, ZB_TILE_SMEM, st>>>(src, place, status, blocks,
-                                                                                                 seqs, lits, dst, first, end, dict);
+    ZB_LAUNCH(zb_execute_tile, (n + ZB_TILE_WARPS - 1) / ZB_TILE_WARPS, ZB_TILE_WARPS * 32, ZB_TILE_SMEM, st, src, place, status, blocks,
+              seqs, lits, dst, first, end, dict);
     if (blk_last <= blk_first) return;
     cudaMemsetAsync(wave_mem, 0, zb_wave_bytes(n_frames, n_blocks), st);
     ZbWave w;
@@ -1832,40 +1834,39 @@ void zb_launch_execute_big(const u8* src, const ZbFramePlace* place, const u32* 
     w.blk_flag = w.pre_blk + n_frames;
     w.ticket = w.blk_flag + n_blocks;
     u64 grid = blk_last - blk_first; if (grid > n_ctas) grid = n_ctas;
-    zb_execute_big<<<(unsigned)grid, ZB_BIG_NT, ZB_BIG_SMEM, st>>>(src, place, status, blocks, (const ZbBlkDesc*)bdesc, seqs, lits, dst,
-                                                                  blk_first, blk_last, dict, (u64)ZB_TILE_CAP + 1, w);
+    ZB_LAUNCH(zb_execute_big, (unsigned)grid, ZB_BIG_NT, ZB_BIG_SMEM, st, src, place, status, blocks, (const ZbBlkDesc*)bdesc, seqs, lits, dst,
+              blk_first, blk_last, dict, (u64)ZB_TILE_CAP + 1, w);
 }
 
 void zb_launch_execute(const u8* src, const ZbFramePlace* place, const u32* status, const ZbBlock* blocks,
                        const ZbSeq* seqs, const u8* lits, u8* dst, u32 first, u32 end, ZbDictDev dict, cudaStream_t st)
 {
     // frames [first, end).  Frames <= ZB_TILE_CAP bytes are regenerated in shared memory, larger ones straight in HBM/L2
-    cudaFuncSetAttribute(zb_execute_tile, cudaFuncAttributeMaxDynamicSharedMemorySize, ZB_TILE_SMEM);      // per device: cheap, so set on every launch
     u32 const n = end - first;
-    zb_execute_tile<<<(n + ZB_TILE_WARPS - 1) / ZB_TILE_WARPS, ZB_TILE_WARPS * 32, ZB_TILE_SMEM, st>>>(src, place, status, blocks,
-                                                                                                 seqs, lits, dst, first, end, dict);
+    ZB_LAUNCH(zb_execute_tile, (n + ZB_TILE_WARPS - 1) / ZB_TILE_WARPS, ZB_TILE_WARPS * 32, ZB_TILE_SMEM, st, src, place, status, blocks,
+              seqs, lits, dst, first, end, dict);
     u32 const warps_per_cta = 8;
-    zb_execute<<<(n + warps_per_cta - 1) / warps_per_cta, warps_per_cta * 32, 0, st>>>(src, place, status, blocks, seqs,
-                                                                                       lits, dst, first, end, dict, (u64)ZB_TILE_CAP + 1);
+    ZB_LAUNCH(zb_execute, (n + warps_per_cta - 1) / warps_per_cta, warps_per_cta * 32, 0, st, src, place, status, blocks, seqs,
+              lits, dst, first, end, dict, (u64)ZB_TILE_CAP + 1);
 }
 
 void zb_launch_verify(const u8* dst, const ZbFramePlace* place, const u64* out_sizes, const ZbFrameInfo* info, const u32* ck_expect,
                       u32 first, u32 end, u32* status, cudaStream_t st)
 {
     u32 const n = end - first;
-    zb_verify_checksums<<<(n + 127) / 128, 128, 0, st>>>(dst, place, out_sizes, info, ck_expect, first, end, status);
-    zb_verify_checksums_big<<<n < 592 ? n : 592, 256, 0, st>>>(dst, place, out_sizes, info, ck_expect, first, end, status);
+    ZB_LAUNCH(zb_verify_checksums, (n + 127) / 128, 128, 0, st, dst, place, out_sizes, info, ck_expect, first, end, status);
+    ZB_LAUNCH(zb_verify_checksums_big, n < 592 ? n : 592, 256, 0, st, dst, place, out_sizes, info, ck_expect, first, end, status);
 }
 
 void zb_launch_finish(const ZbFramePlace* place, const u64* out_sizes, const u32* status, u32 n, ZbSegment* out_segs,
                       u32* first_error, cudaStream_t st)
 {
-    zb_finish<<<(n + 255) / 256, 256, 0, st>>>(place, out_sizes, status, n, out_segs, first_error);
+    ZB_LAUNCH(zb_finish, (n + 255) / 256, 256, 0, st, place, out_sizes, status, n, out_segs, first_error);
 }
 
 void zb_launch_chain_shift(ZbFramePlace* place, u32 n, u64 carry, cudaStream_t st)
 {
-    zb_chain_shift<<<(n + 1 + 255) / 256, 256, 0, st>>>(place, n + 1, carry);
+    ZB_LAUNCH(zb_chain_shift, (n + 1 + 255) / 256, 256, 0, st, place, n + 1, carry);
 }
 
 void zb_entropy_phase_read(unsigned long long* out8, int reset)
@@ -1890,7 +1891,7 @@ void zb_execute_phase_read(unsigned long long* out4, int reset)
 
 void zb_launch_digest_dict(const u8* dict, u32 n, ZbDictDigest* out, cudaStream_t st)
 {
-    zb_digest_dict<<<1, 32, 0, st>>>(dict, n, out);
+    ZB_LAUNCH(zb_digest_dict, 1, 32, 0, st, dict, n, out);
 }
 
 }  // extern "C"

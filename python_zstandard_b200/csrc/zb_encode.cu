@@ -23,6 +23,16 @@
 // A second kernel lays the frames out tightly (frame header ZSTD_writeFrameHeader :27649).
 #include "zb_common.cuh"
 
+// A kernel's dynamic shared memory.  The CPU build of these sources (ZB_SIMT_EMULATION, tests/simt.h) runs one CTA at a time
+// and points every kernel at simt.h's static buffer.  Defined with the kernels rather than in zb_common.cuh, and word for word
+// the same in zb_decode.cu and zb_encode.cu: host builds of the kernel text that define ZB_SIMT_EMULATION after that header,
+// or that rewrite this declaration line, get the CPU form too.
+#ifdef ZB_SIMT_EMULATION
+#define ZB_DYN_SMEM(name) u8* const name = simt_dyn_smem;
+#else
+#define ZB_DYN_SMEM(name) extern __shared__ __align__(16) u8 name[];
+#endif
+
 // Lock-step marker for the CPU emulation of tests/simt.h (fibers run ahead between warp collectives; the hardware does not).
 // Expands to nothing in the device build.
 #ifndef ZB_SIMT_STEP
@@ -107,10 +117,10 @@ struct ZeChainSeg {
     const u32* prev_tab;                // the previous chunk's index (nullptr: none)
     u32 len, prev_len, log, prev_log;
 };
-#define ZE_CHAIN_STEP 4u                // the index samples every 4th position; backward extension finds the true starts
-// An index slot is keyed on the 8 bytes at a position AND on the position's 4 KiB bucket: in a revision the bytes of
-// position p mostly sit near p in the previous revision, and a lookup probes the buckets around p.  Keyed on the bytes
-// alone, the earliest occurrence of a common 8-byte string (indentation, a keyword) would answer for all of them.
+// The index samples every ZE_CHAIN_STEP-th position (zb_common.cuh).  A slot is keyed on the 8 bytes at a position AND on
+// its 4 KiB bucket: in a revision the bytes of position p mostly sit near p in the previous revision, and a lookup probes the
+// buckets around p.  Keyed on the bytes alone, the earliest occurrence of a common 8-byte string (indentation, a keyword)
+// would answer for all of them.
 #define ZE_CHAIN_BUCKET 12u
 __device__ __forceinline__ u32 ze_chain_slot(u64 v, u32 pos, u32 log)
 {
@@ -592,7 +602,7 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
                    ZeScratch* __restrict__ scratch, u8* __restrict__ slots, u64 slot_bytes,
                    ZeBlockOut* __restrict__ outs, u32* __restrict__ work_counter, ZeDict dict, ZeUpload up, u32* __restrict__ stats = nullptr)
 {
-    extern __shared__ __align__(16) u8 ze_smem_raw[];
+    ZB_DYN_SMEM(ze_smem_raw);
     ZeShared& S = *(ZeShared*)ze_smem_raw;
     ZeScratch& G = PREFIX ? (ZeScratch&)((ZePScratch*)scratch)[blockIdx.x] : scratch[blockIdx.x];
     ZePScratch& GP = (ZePScratch&)G;            // (PREFIX only)
@@ -1574,7 +1584,7 @@ extern "C" {
 
 size_t zb_encode_scratch_bytes() { return sizeof(ZeScratch); }
 
-void zb_launch_dict_table(const u8* tail, u32 D, u16* table, cudaStream_t st) { zb_dict_table<<<1, 32, 0, st>>>(tail, D, table); }
+void zb_launch_dict_table(const u8* tail, u32 D, u16* table, cudaStream_t st) { ZB_LAUNCH(zb_dict_table, 1, 32, 0, st, tail, D, table); }
 
 void zb_launch_compress_blocks(const u8* src, const void* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes,
                                void* outs, u32* work_counter, const u8* dict_tail, u32 dict_D, const u16* dict_table, const void* dict_digest, const void* dict_cct,
@@ -1583,17 +1593,15 @@ void zb_launch_compress_blocks(const u8* src, const void* jobs, u32 n_jobs, void
 {
     ZeDict dict; dict.tail = dict_tail; dict.D = dict_D; dict.pad = 0; dict.table = dict_table; dict.ent = (const ZbDictDigest*)dict_digest; dict.cct = dict_digest ? dict_cct : nullptr;
     ZeUpload up; up.progress = upload_progress; up.total = upload_total; up.status = upload_status;
-    #define ZE_LAUNCH(D_, U_, S_) do { \
-        cudaFuncSetAttribute(zb_compress_blocks<D_, U_, S_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ZeShared));   /* per device: cheap, so set on every launch */ \
-        zb_compress_blocks<D_, U_, S_><<<n_ctas, ZE_THREADS, sizeof(ZeShared), st>>>(src, (const ZeBlockJob*)jobs, n_jobs, (ZeScratch*)scratch, slots, slot_bytes, \
-                                                                                     (ZeBlockOut*)outs, work_counter, dict, up, stats); } while (0)
-    if (stats) {        // dictionary training: the statistics of ZDICT_countEStats
-        if (dual) { if (small_blocks) ZE_LAUNCH(true, ZE_UNIT_SMALL, true); else ZE_LAUNCH(true, ZE_UNIT, true); }
-        else      { if (small_blocks) ZE_LAUNCH(false, ZE_UNIT_SMALL, true); else ZE_LAUNCH(false, ZE_UNIT, true); }
-    }
-    else if (dual) { if (small_blocks) ZE_LAUNCH(true, ZE_UNIT_SMALL, false); else ZE_LAUNCH(true, ZE_UNIT, false); }
-    else           { if (small_blocks) ZE_LAUNCH(false, ZE_UNIT_SMALL, false); else ZE_LAUNCH(false, ZE_UNIT, false); }
-    #undef ZE_LAUNCH
+    // the instantiation: two hash tables from level 4 on, 256-byte parse units for small blocks, statistics for dictionary
+    // training (ZDICT_countEStats)
+    decltype(&zb_compress_blocks<false, ZE_UNIT, false>) k;
+    if (stats) k = dual ? (small_blocks ? zb_compress_blocks<true, ZE_UNIT_SMALL, true> : zb_compress_blocks<true, ZE_UNIT, true>)
+                        : (small_blocks ? zb_compress_blocks<false, ZE_UNIT_SMALL, true> : zb_compress_blocks<false, ZE_UNIT, true>);
+    else k = dual ? (small_blocks ? zb_compress_blocks<true, ZE_UNIT_SMALL, false> : zb_compress_blocks<true, ZE_UNIT, false>)
+                  : (small_blocks ? zb_compress_blocks<false, ZE_UNIT_SMALL, false> : zb_compress_blocks<false, ZE_UNIT, false>);
+    ZB_LAUNCH(k, n_ctas, ZE_THREADS, sizeof(ZeShared), st, src, (const ZeBlockJob*)jobs, n_jobs, (ZeScratch*)scratch, slots, slot_bytes,
+              (ZeBlockOut*)outs, work_counter, dict, up, stats);
 }
 
 // content-dictionary chains: the chunk indexes of a run, and its block jobs through the prefix mode
@@ -1603,32 +1611,31 @@ void zb_launch_chain_index(const u8* src, const void* segs, const u64* pos_off, 
 {
     if (!total_pos) return;
     u64 const want = (total_pos + 255) / 256; u32 const grid = (u32)(want < (u64)sms * 16 ? want : (u64)sms * 16);
-    zb_chain_index<<<grid, 256, 0, st>>>(src, (const ZeChainSeg*)segs, pos_off, n_segs);
+    ZB_LAUNCH(zb_chain_index, grid, 256, 0, st, src, (const ZeChainSeg*)segs, pos_off, n_segs);
 }
 void zb_launch_compress_chain_blocks(const u8* src, const void* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes,
                                      void* outs, u32* work_counter, const void* segs, cudaStream_t st)
 {
     ZeDict dict; memset(&dict, 0, sizeof dict); dict.cct = segs;
     ZeUpload up; up.progress = nullptr; up.total = 0; up.status = nullptr;
-    cudaFuncSetAttribute(zb_compress_blocks<false, ZE_UNIT, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ZeShared));
-    zb_compress_blocks<false, ZE_UNIT, false, true><<<n_ctas, ZE_THREADS, sizeof(ZeShared), st>>>(src, (const ZeBlockJob*)jobs, n_jobs, (ZeScratch*)scratch,
-                                                                                            slots, slot_bytes, (ZeBlockOut*)outs, work_counter, dict, up, nullptr);
+    ZB_LAUNCH((zb_compress_blocks<false, ZE_UNIT, false, true>), n_ctas, ZE_THREADS, sizeof(ZeShared), st, src, (const ZeBlockJob*)jobs, n_jobs,
+              (ZeScratch*)scratch, slots, slot_bytes, (ZeBlockOut*)outs, work_counter, dict, up, nullptr);
 }
 
 void zb_launch_frame_layout(const ZbSegment* segs, const void* seginfo, const void* outs, u32 n_segs, u32 checksum, u32 content_size,
                             u32 dict_id, u32 window_log, u64* sizes, ZbSegment* out_segs, u64* total, cudaStream_t st)
 {
     ZeParams P; P.checksum = checksum; P.content_size = content_size; P.dict_id = dict_id; P.level = 3; P.window_log = window_log;
-    zb_frame_sizes<<<(n_segs + 255) / 256, 256, 0, st>>>(segs, (const ZeSegInfo*)seginfo, (const ZeBlockOut*)outs, n_segs, P, sizes);
-    zb_scan_sizes<<<1, 1024, 0, st>>>(sizes, n_segs, out_segs, total);
+    ZB_LAUNCH(zb_frame_sizes, (n_segs + 255) / 256, 256, 0, st, segs, (const ZeSegInfo*)seginfo, (const ZeBlockOut*)outs, n_segs, P, sizes);
+    ZB_LAUNCH(zb_scan_sizes, 1, 1024, 0, st, sizes, n_segs, out_segs, total);
 }
 
 void zb_launch_write_frames(const u8* src, const ZbSegment* segs, const void* seginfo, const void* outs, const u8* slots, u64 slot_bytes,
                             u32 n_segs, u32 checksum, u32 content_size, u32 dict_id, u32 window_log, const ZbSegment* out_segs, u8* dst, cudaStream_t st)
 {
     ZeParams P; P.checksum = checksum; P.content_size = content_size; P.dict_id = dict_id; P.level = 3; P.window_log = window_log;
-    zb_write_frames<<<(n_segs + 7) / 8, 256, 0, st>>>(src, segs, (const ZeSegInfo*)seginfo, (const ZeBlockOut*)outs, slots, slot_bytes, n_segs, P,
-                                                      out_segs, dst);
+    ZB_LAUNCH(zb_write_frames, (n_segs + 7) / 8, 256, 0, st, src, segs, (const ZeSegInfo*)seginfo, (const ZeBlockOut*)outs, slots, slot_bytes, n_segs, P,
+              out_segs, dst);
 }
 
 u32 zb_encode_smem_bytes() { return (u32)sizeof(ZeShared); }
@@ -1640,8 +1647,8 @@ void zb_launch_compress_smem(const u8* src, const void* jobs, u32 n_jobs, void* 
                              const unsigned long long* upload_progress, unsigned long long upload_total, u32* upload_status, cudaStream_t st)
 {
     ZeUpload up; up.progress = upload_progress; up.total = upload_total; up.status = upload_status;
-    cudaFuncSetAttribute(zb_compress_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Z2Shared));
-    zb_compress_smem<<<n_ctas, Z2_NT, sizeof(Z2Shared), st>>>(src, (const ZeBlockJob*)jobs, n_jobs, (Z2Scratch*)scratch, slots, slot_bytes, (ZeBlockOut*)outs, work_counter, up);
+    ZB_LAUNCH(zb_compress_smem, n_ctas, Z2_NT, sizeof(Z2Shared), st, src, (const ZeBlockJob*)jobs, n_jobs, (Z2Scratch*)scratch, slots, slot_bytes,
+              (ZeBlockOut*)outs, work_counter, up);
 }
 u32 zb_encode_small_max() { return ZE_SMALL_MAX; }
 
@@ -1654,11 +1661,11 @@ void zb_launch_compress_recs(const u8* src, const void* jobs, u32 n_jobs, u32 n_
 {
     ZeDict dict; dict.tail = dict_tail; dict.D = dict_D; dict.pad = 0; dict.table = dict_table; dict.ent = (const ZbDictDigest*)dict_digest; dict.cct = dict_cct;
     ZeUpload up; up.progress = upload_progress; up.total = upload_total; up.status = upload_status;
-    cudaFuncSetAttribute(zb_compress_recs, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Z3Shared));
-    zb_compress_recs<<<n_ctas, Z3_NT, sizeof(Z3Shared), st>>>(src, (const ZeBlockJob*)jobs, n_jobs, slots, slot_bytes, (ZeBlockOut*)outs, work_counter, dict, up);
+    ZB_LAUNCH(zb_compress_recs, n_ctas, Z3_NT, sizeof(Z3Shared), st, src, (const ZeBlockJob*)jobs, n_jobs, slots, slot_bytes, (ZeBlockOut*)outs, work_counter,
+              dict, up);
 }
 u32 zb_encode_ctable_bytes() { return (u32)sizeof(ZeCTable); }
-void zb_launch_dict_ctables(const void* digest, void* out3, cudaStream_t st) { zb_dict_ctables<<<1, 96, 0, st>>>((const ZbDictDigest*)digest, (ZeCTable*)out3); }
+void zb_launch_dict_ctables(const void* digest, void* out3, cudaStream_t st) { ZB_LAUNCH(zb_dict_ctables, 1, 96, 0, st, (const ZbDictDigest*)digest, (ZeCTable*)out3); }
 
 void zb_encode_phase_read(unsigned long long* out16, int reset)
 {

@@ -374,7 +374,7 @@ __global__ void __launch_bounds__(Z2_NT, 1)
 zb_compress_smem(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jobs, u32 n_jobs, Z2Scratch* __restrict__ scratch,
                  u8* __restrict__ slots, u64 slot_bytes, ZeBlockOut* __restrict__ outs, u32* __restrict__ work_counter, ZeUpload up)
 {
-    extern __shared__ __align__(16) u8 z2_smem_raw[];
+    ZB_DYN_SMEM(z2_smem_raw);
     Z2Shared& S = *(Z2Shared*)z2_smem_raw;
     Z2Scratch& G = scratch[blockIdx.x];
     u32 const tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;

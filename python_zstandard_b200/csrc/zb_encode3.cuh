@@ -48,7 +48,7 @@ __global__ void __launch_bounds__(Z3_NT, 1)
 zb_compress_recs(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jobs, u32 n_jobs, u8* __restrict__ slots, u64 slot_bytes,
                  ZeBlockOut* __restrict__ outs, u32* __restrict__ work_counter, ZeDict dict, ZeUpload up)
 {
-    extern __shared__ __align__(16) u8 z3_smem_raw[];
+    ZB_DYN_SMEM(z3_smem_raw);
     Z3Shared& S = *(Z3Shared*)z3_smem_raw;
     u32 const tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const ZbDictDigest* const de = dict.ent;

@@ -409,7 +409,7 @@ zb_entropy_decode(const u8* __restrict__ src, const ZbSegment* __restrict__ segs
                   u32* __restrict__ work_counter, ZbDictDev dict, u32* status, u64* __restrict__ out_sizes,
                   u32* __restrict__ ck_expect, u32 take)
 {
-    extern __shared__ __align__(16) u8 zb_smem[];
+    ZB_DYN_SMEM(zb_smem);
     u32 const lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     u32 const pool_bytes = zb_ent_head<ZB_ENT_WARPS>(zb_smem, dict);
     u8* const pool = zb_smem + ZB_ENT_SMEM(ZB_ENT_WARPS) - (ZB_ENT_WARPS - warp) * pool_bytes;      // pools: behind the head
@@ -628,7 +628,7 @@ zb_entropy_blocks(const u8* __restrict__ src, const ZbBlkDesc* __restrict__ bdes
                   ZbBlock* __restrict__ blocks, ZbSeq* __restrict__ seqs, u8* __restrict__ lits,
                   u32* __restrict__ work_counter, ZbDictDev dict, u32* status, ZbBlkExit* __restrict__ bexit, u32 take)
 {
-    extern __shared__ __align__(16) u8 zb_smem[];
+    ZB_DYN_SMEM(zb_smem);
     u32 const lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     u32 const pool_bytes = zb_ent_head<ZB_ENT_WARPS>(zb_smem, dict);
     u8* const pool = zb_smem + ZB_ENT_SMEM(ZB_ENT_WARPS) - (ZB_ENT_WARPS - warp) * pool_bytes;      // pools: behind the head

@@ -251,26 +251,26 @@ extern "C" {
 
 void zt_launch_hash(const u8* s, u32 n_dmers, u32 f, u32 d, u32* hash, u32 sms, cudaStream_t st)
 {
-    zt_hash_all<<<sms * 8, 256, 0, st>>>(s, n_dmers, f, d, hash);
+    ZB_LAUNCH(zt_hash_all, sms * 8, 256, 0, st, s, n_dmers, f, d, hash);
 }
 void zt_launch_count(const u32* hash, const u64* offs, u32 n_train, u32 step, u32* freqs, u32 sms, cudaStream_t st)
 {
-    zt_count<<<sms * 8, 256, 0, st>>>(hash, offs, n_train, step, freqs);
+    ZB_LAUNCH(zt_count, sms * 8, 256, 0, st, hash, offs, n_train, step, freqs);
 }
 void zt_launch_prev(const u32* hash, u32 n, u32* prev, u8* last, u32* table, cudaStream_t st)
 {
-    zt_prev_local<<<(n + ZT_CHUNK - 1) / ZT_CHUNK, 1024, 0, st>>>(hash, n, prev, last);
-    zt_prev_link<<<1, 1024, 0, st>>>(hash, n, prev, last, table);
+    ZB_LAUNCH(zt_prev_local, (n + ZT_CHUNK - 1) / ZT_CHUNK, 1024, 0, st, hash, n, prev, last);
+    ZB_LAUNCH(zt_prev_link, 1, 1024, 0, st, hash, n, prev, last, table);
 }
-void zt_launch_select(const void* a, u32 n_ctas, cudaStream_t st) { zt_select<<<n_ctas, 1024, 0, st>>>(*(const ZtSelect*)a); }
+void zt_launch_select(const void* a, u32 n_ctas, cudaStream_t st) { ZB_LAUNCH(zt_select, n_ctas, 1024, 0, st, *(const ZtSelect*)a); }
 void zt_launch_entropy(const u32* stats, u32 content_size, u8* ent, u32* ent_len, cudaStream_t st)
 {
-    zt_entropy<<<1, 32, 0, st>>>(stats, content_size, ent, ent_len);
+    ZB_LAUNCH(zt_entropy, 1, 32, 0, st, stats, content_size, ent, ent_len);
 }
 void zt_launch_finalize(const u8* dict, u32 cap, const u32* tail, const u8* ent, const u32* ent_len, u32 dict_id, u8* out, long long* res,
                         cudaStream_t st)
 {
-    zt_finalize<<<1, 256, 0, st>>>(dict, cap, tail, ent, ent_len, dict_id, out, res);
+    ZB_LAUNCH(zt_finalize, 1, 256, 0, st, dict, cap, tail, ent, ent_len, dict_id, out, res);
 }
 
 }  // extern "C"

@@ -12,7 +12,8 @@ import subprocess
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-SRC = os.path.join(ROOT, "python_zstandard_b200", "csrc", "zb_encode.cu")
+CSRC = os.path.join(ROOT, "python_zstandard_b200", "csrc")
+SRC = os.path.join(CSRC, "zb_encode.cu")
 BUILD = os.path.join(HERE, "_build")
 LIB = os.path.join(BUILD, "libze_host.so")
 
@@ -154,288 +155,52 @@ def build_header_parser():
     return L
 
 
-SIM_LIB = os.path.join(BUILD, "libzs_host.so")
-SIM_WRAPPERS = r"""
-extern "C" unsigned long long t_any_calls(int reset) { unsigned long long v = simt_any_calls; if (reset) simt_any_calls = 0; return v; }
-// The whole compression path of the library on the CPU: block jobs cut as zb_api.cu cuts them (zb_cut_blocks, blocks of
-// min(2^window_log, 128 KiB)), zb_compress_blocks on `n_ctas` CTAs of 128 threads -- the two-table instantiation from level 4
-// on, as the launcher picks it -- or zb_compress_recs when `recs` is set, then the frame layout kernels with the level and
-// window_log of the call.  Input resident.  Returns total bytes.
-extern "C" long long t_compress_batch(const u8* src, const u64* seg_off, const u64* seg_len, u32 n_segs, u32 checksum, u32 content_size,
-                                      u32 n_ctas, u8* out, u64 out_cap, u64* out_off, u64* out_len, u32 recs, const u8* dict_raw, u32 dict_n,
-                                      int level, u32 window_log)
-{
-    std::vector<ZbSegment> segs(n_segs); std::vector<ZeBlockJob> jobs; std::vector<ZeSegInfo> info(n_segs);
-    for (u32 i = 0; i < n_segs; i++) { segs[i].offset = seg_off[i]; segs[i].length = seg_len[i]; }
-    u32 const max_block = zb_cut_blocks(segs.data(), n_segs, zb_block_max(window_log), jobs, info);
-    bool const dual = level >= 4;
-    u32 const nj = (u32)jobs.size();
-    u64 const slot_bytes = ((u64)max_block + (max_block >> 7) + 64 + 15) & ~15ull;
-    std::vector<u8> slots((size_t)(nj + 1) * slot_bytes); std::vector<ZeBlockOut> outs(nj + 1);
-    if (n_ctas > nj) n_ctas = nj ? nj : 1;
-    ZeScratch* scratch = (ZeScratch*)aligned_alloc(64, ((sizeof(ZeScratch) + 63) & ~(size_t)63) * n_ctas);
-    u32 counter = 0;
-    ZeDict dict; memset(&dict, 0, sizeof dict);
-    static ZbDictDigest dg; static u16 dtable[1 << ZE_HLOG]; static ZeCTable cct[3];
-    u32 dict_id = 0;
-    if (dict_raw && dict_n) {          // what zb200_ddict_create does: digest, compression view (last <= 32 KiB), hash table, CTables
-        simt::launch(1, 32, [&] { zb_digest_dict(dict_raw, dict_n, &dg); });
-        if (dg.status != ZB_OK) return -2;
-        const u8* content = dg.has_entropy ? dict_raw + dg.content_off : dict_raw;
-        u32 const csize = dg.has_entropy ? dict_n - dg.content_off : dict_n;
-        u32 const D = csize < 32768u ? csize : 32768u;
-        if (D >= 8) {
-            dict.tail = content + (csize - D); dict.D = D; dict.table = dtable; dict_id = dg.dict_id;
-            simt::launch(1, 32, [&] { zb_dict_table(dict.tail, D, dtable); });
-            if (dg.has_entropy) { dict.ent = &dg; dict.cct = cct; simt::launch(1, 96, [&] { zb_dict_ctables(&dg, cct); }); }
-        }
-    }
-    ZeUpload up; up.progress = nullptr; up.total = 0; up.status = nullptr;
-    ZeParams P; P.checksum = checksum; P.content_size = content_size; P.dict_id = dict_id; P.level = (u32)level; P.window_log = window_log;
-    bool const small_blocks = max_block <= ZE_SMALL_MAX;             // as zb_api.cu picks the instantiation
-    if (nj && recs) simt::launch((nj + Z3_WARPS - 1) / Z3_WARPS < n_ctas ? (nj + Z3_WARPS - 1) / Z3_WARPS : n_ctas, Z3_NT, [&] { zb_compress_recs(src, jobs.data(), nj, slots.data(), slot_bytes, outs.data(), &counter, dict, up); });
-    else if (nj && dual && small_blocks) simt::launch(n_ctas, ZE_THREADS, [&] { zb_compress_blocks<true, ZE_UNIT_SMALL>(src, jobs.data(), nj, (ZeScratch*)scratch, slots.data(), slot_bytes, outs.data(), &counter, dict, up); });
-    else if (nj && small_blocks) simt::launch(n_ctas, ZE_THREADS, [&] { zb_compress_blocks<false, ZE_UNIT_SMALL>(src, jobs.data(), nj, (ZeScratch*)scratch, slots.data(), slot_bytes, outs.data(), &counter, dict, up); });
-    else if (nj && dual) simt::launch(n_ctas, ZE_THREADS, [&] { zb_compress_blocks<true, ZE_UNIT>(src, jobs.data(), nj, (ZeScratch*)scratch, slots.data(), slot_bytes, outs.data(), &counter, dict, up); });
-    else if (nj) simt::launch(n_ctas, ZE_THREADS, [&] { zb_compress_blocks<false, ZE_UNIT>(src, jobs.data(), nj, (ZeScratch*)scratch, slots.data(), slot_bytes, outs.data(), &counter, dict, up); });
-    std::vector<u64> sizes(n_segs); std::vector<ZbSegment> out_segs(n_segs); u64 total = 0;
-    simt::launch((n_segs + 255) / 256, 256, [&] { zb_frame_sizes(segs.data(), info.data(), outs.data(), n_segs, P, sizes.data()); });
-    simt::launch(1, 1024, [&] { zb_scan_sizes(sizes.data(), n_segs, out_segs.data(), &total); });
-    free(scratch);
-    if (total > out_cap) return -1;
-    simt::launch((n_segs + 7) / 8, 256, [&] { zb_write_frames(src, segs.data(), info.data(), outs.data(), slots.data(), slot_bytes, n_segs, P, out_segs.data(), out); });
-    for (u32 i = 0; i < n_segs; i++) { out_off[i] = out_segs[i].offset; out_len[i] = out_segs[i].length; }
-    return (long long)total;
-}
-
-// The round-2 kernel (zb_compress_smem: one CTA of 1024 threads per block, block resident in "shared memory") on the CPU,
-// with the jobs and frame headers of a call with this level and window_log.
-extern "C" long long t_compress_batch2(const u8* src, const u64* seg_off, const u64* seg_len, u32 n_segs, u32 checksum, u32 content_size,
-                                       u32 n_ctas, u8* out, u64 out_cap, u64* out_off, u64* out_len, int level, u32 window_log)
-{
-    std::vector<ZbSegment> segs(n_segs); std::vector<ZeBlockJob> jobs; std::vector<ZeSegInfo> info(n_segs);
-    for (u32 i = 0; i < n_segs; i++) { segs[i].offset = seg_off[i]; segs[i].length = seg_len[i]; }
-    u32 const max_block = zb_cut_blocks(segs.data(), n_segs, zb_block_max(window_log), jobs, info);
-    u32 const nj = (u32)jobs.size();
-    u64 const slot_bytes = ((u64)max_block + (max_block >> 7) + 64 + 15) & ~15ull;
-    u8* slots = (u8*)aligned_alloc(64, (size_t)(nj + 1) * slot_bytes + 64); std::vector<ZeBlockOut> outs(nj + 1);
-    if (n_ctas > nj) n_ctas = nj ? nj : 1;
-    Z2Scratch* scratch = (Z2Scratch*)aligned_alloc(64, ((sizeof(Z2Scratch) + 63) & ~(size_t)63) * n_ctas);
-    u32 counter = 0;
-    ZeUpload up; up.progress = nullptr; up.total = 0; up.status = nullptr;
-    ZeParams P; P.checksum = checksum; P.content_size = content_size; P.dict_id = 0; P.level = (u32)level; P.window_log = window_log;
-    if (nj) simt::launch(n_ctas, Z2_NT, [&] { zb_compress_smem(src, jobs.data(), nj, scratch, slots, slot_bytes, outs.data(), &counter, up); });
-    std::vector<u64> sizes(n_segs); std::vector<ZbSegment> out_segs(n_segs); u64 total = 0;
-    simt::launch((n_segs + 255) / 256, 256, [&] { zb_frame_sizes(segs.data(), info.data(), outs.data(), n_segs, P, sizes.data()); });
-    simt::launch(1, 1024, [&] { zb_scan_sizes(sizes.data(), n_segs, out_segs.data(), &total); });
-    free(scratch);
-    if (total > out_cap) { free(slots); return -1; }
-    simt::launch((n_segs + 7) / 8, 256, [&] { zb_write_frames(src, segs.data(), info.data(), outs.data(), slots, slot_bytes, n_segs, P, out_segs.data(), out); });
-    free(slots);
-    for (u32 i = 0; i < n_segs; i++) { out_off[i] = out_segs[i].offset; out_len[i] = out_segs[i].length; }
-    return (long long)total;
-}
-"""
+SIM_SRC = os.path.join(HERE, "simt_kernels.cpp")
+SIM_LIB = os.path.join(BUILD, "libzsim.so")
+# The CPU build of the kernels: simt.h's runtime, the compressor's lock-step markers, and the decoder's big-frame thresholds
+# lowered from 512 KiB / 256 KiB so that small test frames reach the warp-cooperative scans and checksums.
+SIM_FLAGS = ["-DZB_SIMT_EMULATION", "-DZB_SIMT_STEP()=__syncwarp()", "-DZB_SCAN_BIG=24000u", "-DZB_XXH_BIG=50000u"]
 
 
-def build_compress_sim():
-    """Host build of the whole compression kernel source (zb_encode.cu up to its launchers) on the mini SIMT runtime of
-    tests/simt.h: 128 fibers per CTA, warp collectives and barriers as rendezvous."""
-    os.makedirs(BUILD, exist_ok=True)
-    import re
-    csrc = os.path.join(ROOT, "python_zstandard_b200", "csrc")
-    enc = open(SRC).read()
-    a = enc.index('#include "zb_common.cuh"')
-    a = enc.index("\n", a) + 1
-    b = enc.index('extern "C" {')
-    b = enc.rindex("// ====", 0, enc.rindex("// ====", 0, b))
-    body = enc[a:b].replace('#include "zb_encode2.cuh"', open(os.path.join(csrc, "zb_encode2.cuh")).read().replace("#pragma once", ""))
-    body = body.replace('#include "zb_encode3.cuh"', open(os.path.join(csrc, "zb_encode3.cuh")).read().replace("#pragma once", ""))
-    dec = open(os.path.join(csrc, "zb_decode.cu")).read()
-    da = dec.index("\n", dec.index('#include "zb_common.cuh"')) + 1
-    db = dec.index('extern "C" {')
-    db = dec.rindex("// ====", 0, dec.rindex("// ====", 0, db))
-    dbody = dec[da:db].replace('#include "zb_entropy.cuh"', open(DEC_SRC).read().replace("#pragma once", ""))
-    body = dbody + body                                      # the dictionary digest lives with the decoder
-    body = re.sub(r"extern __shared__ __align__\(16\) u8 (\w+)\[\];", r"u8* const \1 = simt_dyn_smem;", body)
-    text = (LIT_PRELUDE + "#include <cmath>\n#include <vector>\n" + '#include "%s"\n' % os.path.join(csrc, "zb_common.cuh")
-            + '#include "%s"\n' % os.path.join(HERE, "simt.h") + "alignas(16) static u8 simt_dyn_smem[256 << 10];\n#define ZB_SIMT_STEP() __syncwarp()\n#define ZB_SIMT_EMULATION 1\n" + body + SIM_WRAPPERS)
-    cpp = os.path.join(BUILD, "zs_host.cpp")
-    if not (os.path.exists(SIM_LIB) and os.path.exists(cpp) and open(cpp).read() == text
-            and os.path.getmtime(SIM_LIB) >= os.path.getmtime(os.path.join(HERE, "simt.h"))):
-        open(cpp, "w").write(text)
-        subprocess.check_call(["g++", "-std=c++17", "-O1", "-shared", "-fPIC", "-I/usr/local/cuda/include", "-o", SIM_LIB, cpp])
-    L = C.CDLL(SIM_LIB)
+def build_sim(lib=SIM_LIB, extra=()):
+    """Host build of the whole kernel source -- zb_decode.cu and zb_encode.cu as they are, launchers included -- on the mini
+    SIMT runtime of tests/simt.h, with the wrappers of tests/simt_kernels.cpp.  `extra`: more g++ flags (sanitizers)."""
+    import glob
+    import hashlib
+    os.makedirs(os.path.dirname(lib), exist_ok=True)
+    # -Bsymbolic: the library's calls bind to its own definitions -- simt.h's cudaMemsetAsync and the launchers -- even
+    # when the process has loaded the CUDA runtime or libzb200.so, which export the same names
+    cmd = (["g++", "-std=c++17", "-O2", "-shared", "-fPIC", "-Wl,-Bsymbolic", "-I/usr/local/cuda/include", "-I" + CSRC, "-I" + HERE]
+           + SIM_FLAGS + list(extra) + [SIM_SRC])
+    h = hashlib.sha256(" ".join(cmd).encode())
+    for f in sorted(glob.glob(os.path.join(CSRC, "*.cu*"))) + [SIM_SRC, os.path.join(HERE, "simt.h")]:
+        h.update(open(f, "rb").read())
+    stamp = lib + ".sha256"
+    if not (os.path.exists(lib) and os.path.exists(stamp) and open(stamp).read() == h.hexdigest()):
+        tmp = "%s.%d.tmp" % (lib, os.getpid())          # processes that build at once each replace the library whole
+        subprocess.check_call(cmd + ["-o", tmp])
+        os.replace(tmp, lib)
+        open(stamp, "w").write(h.hexdigest())
+    L = C.CDLL(lib)
+    vp, u32, u64, i32 = C.c_void_p, C.c_uint32, C.c_uint64, C.c_int
+    L.t_any_calls.restype = C.c_ulonglong
     L.t_compress_batch.restype = C.c_longlong
-    L.t_compress_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
-                                   C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32,
-                                   C.c_int, C.c_uint32]
+    L.t_compress_batch.argtypes = [vp, vp, vp, u32, u32, u32, u32, vp, u64, vp, vp, u32, vp, u32, i32, u32]
     L.t_compress_batch2.restype = C.c_longlong
-    L.t_compress_batch2.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
-                                    C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_int, C.c_uint32]
-    return L
-
-
-DSIM_LIB = os.path.join(BUILD, "libzd_sim.so")
-DSIM_WRAPPERS = r"""
-// The whole decompression path on the CPU, kernel by kernel as zb_api.cu launches them: scan, placement (reduce + scan),
-// the lane-per-frame entropy kernel on `n_ctas` CTAs of `warps` warps with `take` frames per warp, both execute kernels,
-// checksum verification, finish.  Output: tightly packed bytes + per-frame {offset, length}, status[] per frame.
-static int g_block_path = 0;
-extern "C" void t_set_block_path(int on) { g_block_path = on; }
-// The frame scans (small frames a thread each, big ones a warp each) and the placement, as zb_api.cu runs them before it
-// chooses a path: totals_out[0..5] = output, blocks, sequences, literals, any checksum, any window >= ZB_FAR_WINDOW.
-extern "C" void t_scan_totals(const u8* src, const u64* seg_off, const u64* seg_len, u32 n, u64* totals_out)
-{
-    std::vector<ZbSegment> segs(n); for (u32 i = 0; i < n; i++) { segs[i].offset = seg_off[i]; segs[i].length = seg_len[i]; }
-    std::vector<ZbFrameInfo> info(n); std::vector<ZbFramePlace> place(n + 1); std::vector<u32> status(n, 0), big(n + 1, 0);
-    u64 totals[8] = {0}; u32 const pctas = (n + ZB_PLACE_CTA - 1) / ZB_PLACE_CTA; std::vector<u64> partial(pctas * 4 + 4);
-    simt::launch((n + 127) / 128, 128, [&] { zb_scan_frames(src, segs.data(), n, info.data(), (1ull << 27) + 1, big.data()); });
-    simt::launch(n < 128 ? (n + 3) / 4 : 32, 128, [&] { zb_scan_frames_big(src, segs.data(), big.data(), info.data()); });
-    simt::launch(pctas, ZB_PLACE_CTA, [&] { zb_place_reduce(info.data(), nullptr, n, partial.data()); });
-    simt::launch(pctas, ZB_PLACE_CTA, [&] { zb_place_scan(info.data(), nullptr, n, partial.data(), place.data(), totals, status.data()); });
-    for (int k = 0; k < 6; k++) totals_out[k] = totals[k];
-}
-// `chunk_bytes` 0: one chunk of all frames, the entropy kernel on `n_ctas` CTAs of `warps` warps with `take` frames per warp.
-// Otherwise the call is cut as run_decompress cuts a call whose output is copied back (zb_chunk_count with this chunk size,
-// zb_chunk_cut), and every chunk runs what the launcher runs for it: the lane-per-frame entropy kernel over frames
-// [0, cut[k + 1]) from a counter of its own that starts at cut[k], shaped by zb_chunk_shape from the chunk's output bytes
-// with `n_ctas` as the SM count (the block path keeps its one entropy launch for all blocks); then the chunk's execute stage
-// -- zb_execute_tile + zb_execute over its frames, zb_execute_big over its blocks with a fresh wave, or the pointer-jumping
-// rounds over its output bytes -- and its checksums.  The pointer-jumping stage regenerates every frame itself, small ones
-// included: as in zb_launch_execute_chase, no tile executor runs in front of it.
-// The copy of chunk k overlaps the kernels of chunk k + 1 on the device.  Here the chunk's output range is copied into `out`
-// as soon as its kernels are done, and is then overwritten in the working buffer with bytes that differ from every output
-// byte (the copy may read at any moment, and no kernel of a later chunk may read or write there).  `out` holds nothing but
-// these copies.  The chunk's regenerated sizes are set aside the same way until zb_finish: a later chunk must not decode
-// its frames again.  plan (nullable, 3 + 5 * 33 words): n_chunks, bytes of earlier chunks that later chunks wrote, frames
-// of earlier chunks that later chunks decoded again; then per chunk {cut, warps, take, ctas, output bytes}, where warps, take
-// and ctas are those of the chunk's lane-per-frame entropy launch (0 on the block path, whose one launch is not per chunk).
-extern "C" long long t_decompress_batch(const u8* src, const u64* seg_off, const u64* seg_len, u32 n, const u8* dict_raw, u32 dict_n,
-                                        u32 n_ctas, u32 warps, u32 take, u8* out, u64 out_cap, u64* out_off, u64* out_len, u32* status_out,
-                                        const u64* dst_sizes /* nullable: the decompressed_sizes argument of the batch call */,
-                                        u64 chunk_bytes, u64* plan)
-{
-    static bool tables = false;
-    if (!tables) { simt::launch(1, 32, [] { zb_build_default_tables(); }); tables = true; }
-    static ZbDictDigest dg; ZbDictDev dict; memset(&dict, 0, sizeof dict);
-    if (dict_raw && dict_n) {
-        simt::launch(1, 32, [&] { zb_digest_dict(dict_raw, dict_n, &dg); });
-        if (dg.status != ZB_OK) return -(long long)dg.status;
-        if (dg.has_entropy) {
-            dict.content = dict_raw + dg.content_off; dict.content_size = dict_n - dg.content_off; dict.dict_id = dg.dict_id; dict.has_entropy = 1;
-            dict.huf = dg.huf; dict.huf_log = dg.huf_log; dict.ll = dg.ll; dict.of = dg.of; dict.ml = dg.ml;
-            dict.ll_log = dg.ll_log; dict.of_log = dg.of_log; dict.ml_log = dg.ml_log;
-            dict.rep[0] = dg.rep[0]; dict.rep[1] = dg.rep[1]; dict.rep[2] = dg.rep[2];
-        } else { dict.content = dict_raw; dict.content_size = dict_n; }
-    }
-    std::vector<ZbSegment> segs(n); for (u32 i = 0; i < n; i++) { segs[i].offset = seg_off[i]; segs[i].length = seg_len[i]; }
-    std::vector<ZbFrameInfo> info(n); std::vector<ZbFramePlace> place(n + 1); std::vector<u32> status(n, 0);
-    u64 totals[8] = {0}; u32 const pctas = (n + ZB_PLACE_CTA - 1) / ZB_PLACE_CTA; std::vector<u64> partial(pctas * 4 + 4);
-    std::vector<u32> big(n + 1, 0);            // frames above ZB_SCAN_BIG (24 KB in this build) are scanned by a warp each
-    simt::launch((n + 127) / 128, 128, [&] { zb_scan_frames(src, segs.data(), n, info.data(), (1ull << 27) + 1, big.data()); });
-    simt::launch(n < 128 ? (n + 3) / 4 : 32, 128, [&] { zb_scan_frames_big(src, segs.data(), big.data(), info.data()); });
-    simt::launch(pctas, ZB_PLACE_CTA, [&] { zb_place_reduce(info.data(), dst_sizes, n, partial.data()); });
-    simt::launch(pctas, ZB_PLACE_CTA, [&] { zb_place_scan(info.data(), dst_sizes, n, partial.data(), place.data(), totals, status.data()); });
-    if (totals[0] > out_cap) return -1000;
-    std::vector<ZbBlock> blocks(totals[1] + 1); std::vector<ZbSeq> seqs(totals[2] + 2); std::vector<u8> lits(totals[3] + 64);
-    std::vector<u64> out_sizes(n, 0); std::vector<u32> ck(n, 0);
-    std::vector<u8> dev(totals[0] + 64, 0); u8* const d_out = dev.data();       // the device's output buffer
-    std::vector<ZbBlkDesc> bdesc;
-    u32 const n_chunks = chunk_bytes ? zb_chunk_count(totals[0], n, true, chunk_bytes) : 1;
-    std::vector<u32> cut(n_chunks + 1); for (u32 k = 0; k <= n_chunks; k++) cut[k] = zb_chunk_cut(n, k, n_chunks);
-    if (g_block_path) {          // a lane per BLOCK: zb_scan_blocks -> zb_entropy_blocks -> zb_resolve_blocks -> zb_patch_blocks
-        u64 const nb = totals[1];
-        u32 const btake = chunk_bytes ? 3 : (take > 3 ? 3 : take);
-        u32 bctas = n_ctas; if (chunk_bytes) { u64 const need = (nb + 7 * btake - 1) / (7 * btake); if (bctas > need) bctas = (u32)need; if (bctas == 0) bctas = 1; }
-        u32 counter = 0;
-        bdesc.resize(nb + 1); std::vector<ZbBlkExit> bexit(nb + 1); std::vector<u32> erep(3 * (nb + 1)); std::vector<u64> fend(n);
-        simt::launch((n + 63) / 64, 64, [&] { zb_scan_blocks(src, segs.data(), n, place.data(), dict, status.data(), bdesc.data(), fend.data(), big.data()); });
-        simt::launch(n < 128 ? (n + 3) / 4 : 32, 128, [&] { zb_scan_blocks_big(src, segs.data(), big.data(), place.data(), dict, status.data(), bdesc.data(), fend.data()); });
-        simt::launch(bctas, 7 * 32, [&] { zb_entropy_blocks<7>(src, bdesc.data(), (u32)nb, blocks.data(), seqs.data(), lits.data(), &counter, dict, status.data(), bexit.data(), btake); });
-        simt::launch((n + 63) / 64, 64, [&] { zb_resolve_blocks(src, segs.data(), n, place.data(), info.data(), dst_sizes, blocks.data(), bdesc.data(), bexit.data(), fend.data(), dict, status.data(), out_sizes.data(), ck.data(), erep.data()); });
-        if (nb) simt::launch((unsigned)((nb + 7) / 8), 256, [&] { zb_patch_blocks(blocks.data(), bdesc.data(), nb, seqs.data(), erep.data(), dict, status.data()); });
-    }
-    std::vector<u32> ptr(g_block_path == 2 ? totals[0] + 16 : 0);
-    u64 changed_bytes = 0, redone = 0;
-    std::vector<u64> sizes_aside(n);
-    std::vector<u8> copy(totals[0] + 64, 0);           // what the copy stream took, chunk by chunk
-    auto poison = [](u64 p) { return (u8)(1 + p % 251); };
-    for (u32 k = 0; k < n_chunks; k++) {
-        u32 const f0 = cut[k], f1 = cut[k + 1];
-        u64 const lo = n_chunks > 1 ? place[f0].dst_off : 0, hi = n_chunks > 1 ? place[f1].dst_off : totals[0];
-        u64 const blo = n_chunks > 1 ? place[f0].blk_off : 0, bhi = n_chunks > 1 ? place[f1].blk_off : totals[1];
-        ZbChunkShape sh; sh.warps = warps; sh.take = take; sh.ctas = n_ctas;
-        if (g_block_path) sh.warps = sh.take = sh.ctas = 0;
-        else if (chunk_bytes) sh = zb_chunk_shape(hi - lo, f1 - f0, n_ctas);
-        if (!g_block_path) {
-            u32 counter = f0;
-            if (sh.warps == 8) simt::launch(sh.ctas, 8 * 32, [&] { zb_entropy_decode<8>(src, segs.data(), f1, place.data(), dst_sizes, blocks.data(), seqs.data(), lits.data(), &counter, dict, status.data(), out_sizes.data(), ck.data(), sh.take); });
-            else simt::launch(sh.ctas, 7 * 32, [&] { zb_entropy_decode<7>(src, segs.data(), f1, place.data(), dst_sizes, blocks.data(), seqs.data(), lits.data(), &counter, dict, status.data(), out_sizes.data(), ck.data(), sh.take); });
-        }
-        if (g_block_path == 2) {     // pointer-jumping execute stage (zb_chase_*): init, doubling rounds until nothing changes, gather
-            if (hi > lo && bhi > blo) {
-                std::fill(ptr.begin() + lo, ptr.begin() + hi, 0xFFFFFFFFu); u32 changed = 0; int rounds = 0;
-                simt::launch(3, 256, [&] { zb_chase_init<u32>(src, place.data(), status.data(), blocks.data(), (const ZbBlkDesc*)bdesc.data(), seqs.data(), lits.data(), d_out, ptr.data(), blo, bhi, dict); });
-                do { changed = 0; simt::launch(4, 256, [&] { zb_chase_round<u32>(ptr.data(), lo, hi, &changed); }); rounds++; } while (changed && rounds < 72);
-                simt::launch(4, 256, [&] { zb_chase_gather<u32>(ptr.data(), d_out, lo, hi, totals[0]); });
-            }
-        }
-        else {
-            simt::launch((f1 - f0 + ZB_TILE_WARPS - 1) / ZB_TILE_WARPS, ZB_TILE_WARPS * 32, [&] { zb_execute_tile(src, place.data(), status.data(), blocks.data(), seqs.data(), lits.data(), d_out, f0, f1, dict); });
-            if (g_block_path && bhi > blo) {
-                std::vector<unsigned long long> w_done(n + 1, 0); std::vector<u32> w_pre(n + 1, 0), w_flag(totals[1] + 1, 0); u32 w_ticket = 0;
-                ZbWave w; w.done_pos = w_done.data(); w.pre_blk = w_pre.data(); w.blk_flag = w_flag.data(); w.ticket = &w_ticket;
-                simt::launch(3, ZB_BIG_NT, [&] { zb_execute_big(src, place.data(), status.data(), blocks.data(), (const ZbBlkDesc*)bdesc.data(), seqs.data(), lits.data(), d_out,
-                                                               blo, bhi, dict, (u64)ZB_TILE_CAP + 1, w); });
-            }
-            else if (!g_block_path) simt::launch((f1 - f0 + 7) / 8, 256, [&] { zb_execute(src, place.data(), status.data(), blocks.data(), seqs.data(), lits.data(), d_out, f0, f1, dict, (u64)ZB_TILE_CAP + 1); });
-        }
-        if (totals[4]) simt::launch((f1 - f0 + 127) / 128, 128, [&] { zb_verify_checksums(d_out, place.data(), out_sizes.data(), info.data(), ck.data(), f0, f1, status.data()); });
-        if (totals[4]) simt::launch(f1 - f0 < 8 ? f1 - f0 : 8, 256, [&] { zb_verify_checksums_big(d_out, place.data(), out_sizes.data(), info.data(), ck.data(), f0, f1, status.data()); });
-        // the copy of the chunk; the working buffer's bytes there are not read again
-        for (u64 p = lo; p < hi; p++) { copy[p] = d_out[p]; d_out[p] ^= poison(p); }
-        for (u32 f = f0; f < f1; f++) { sizes_aside[f] = out_sizes[f]; out_sizes[f] = ~0ull; }
-        if (plan && k < 33) { u64* c = plan + 3 + 5 * k; c[0] = f0; c[1] = sh.warps; c[2] = sh.take; c[3] = sh.ctas; c[4] = hi - lo; }
-    }
-    for (u64 p = 0; p < totals[0]; p++) changed_bytes += d_out[p] != (u8)(copy[p] ^ poison(p));
-    for (u32 f = 0; f < n; f++) { redone += out_sizes[f] != ~0ull; out_sizes[f] = sizes_aside[f]; }
-    memcpy(out, copy.data(), totals[0]);
-    if (plan) { plan[0] = n_chunks; plan[1] = changed_bytes; plan[2] = redone; }
-    std::vector<ZbSegment> out_segs(n); u32 first_error = 0xFFFFFFFFu;
-    simt::launch((n + 255) / 256, 256, [&] { zb_finish(place.data(), out_sizes.data(), status.data(), n, out_segs.data(), &first_error); });
-    for (u32 i = 0; i < n; i++) { out_off[i] = out_segs[i].offset; out_len[i] = out_segs[i].length; status_out[i] = status[i]; }
-    return (long long)totals[0];
-}
-"""
-
-
-def build_decode_sim():
-    """Host build of ALL decompression kernels (zb_decode.cu + zb_entropy.cuh up to the launchers) on tests/simt.h."""
-    import re
-    os.makedirs(BUILD, exist_ok=True)
-    csrc = os.path.join(ROOT, "python_zstandard_b200", "csrc")
-    dec = open(os.path.join(csrc, "zb_decode.cu")).read()
-    a = dec.index('#include "zb_common.cuh"')
-    a = dec.index("\n", a) + 1
-    b = dec.index('extern "C" {')
-    b = dec.rindex("// ====", 0, dec.rindex("// ====", 0, b))
-    body = dec[a:b].replace('#include "zb_entropy.cuh"', open(DEC_SRC).read().replace("#pragma once", ""))
-    body = re.sub(r"extern __shared__ __align__\(16\) u8 (\w+)\[\];", r"u8* const \1 = simt_dyn_smem;", body)
-    text = (LIT_PRELUDE + "#include <cmath>\n#include <vector>\n" + '#include "%s"\n' % os.path.join(csrc, "zb_common.cuh")
-            + '#include "%s"\n' % os.path.join(HERE, "simt.h") + "alignas(16) static u8 simt_dyn_smem[256 << 10];\n#define ZB_SCAN_BIG 24000u\n#define ZB_XXH_BIG 50000u\n" + body + DSIM_WRAPPERS)
-    cpp = os.path.join(BUILD, "zd_sim.cpp")
-    if not (os.path.exists(DSIM_LIB) and os.path.exists(cpp) and open(cpp).read() == text
-            and os.path.getmtime(DSIM_LIB) >= os.path.getmtime(os.path.join(HERE, "simt.h"))):
-        open(cpp, "w").write(text)
-        subprocess.check_call(["g++", "-std=c++17", "-O1", "-shared", "-fPIC", "-I/usr/local/cuda/include", "-o", DSIM_LIB, cpp])
-    L = C.CDLL(DSIM_LIB)
+    L.t_compress_batch2.argtypes = [vp, vp, vp, u32, u32, u32, u32, vp, u64, vp, vp, i32, u32]
+    L.t_compress_chain_run.restype = C.c_longlong
+    L.t_compress_chain_run.argtypes = [vp, vp, vp, u32, u32, u32, vp, u64, vp, vp]
     L.t_decompress_batch.restype = C.c_longlong
-    L.t_decompress_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32,
-                                     C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                     C.c_uint64, C.c_void_p]
+    L.t_decompress_batch.argtypes = [vp, vp, vp, u32, vp, u32, u32, u32, u32, vp, u64, vp, vp, vp, vp, u64, vp]
     L.t_scan_totals.restype = None
-    L.t_scan_totals.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
+    L.t_scan_totals.argtypes = [vp, vp, vp, u32, vp]
+    L.t_decompress_chain_run.restype = C.c_longlong
+    L.t_decompress_chain_run.argtypes = [vp, vp, vp, u32, C.c_char_p, u64, vp, u64, vp, vp, vp, C.POINTER(C.c_int)]
+    L.t_freqs.argtypes = [vp, vp, u32, u32, u32, u32, vp]
+    L.t_prev.argtypes = [vp, u32, u32, vp]
+    L.t_select.argtypes = [vp, vp, u32, u32, u32, u32, u32, u32, vp, vp]
+    L.t_finalize.argtypes = [vp, u32, u32, vp, u32, vp]
+    L.t_finalize.restype = C.c_longlong
     return L
 
 

@@ -7,7 +7,11 @@
 // interleaved instruction by instruction as on the device: code whose RESULT depends on that interleaving (the hash
 // heads of the compressor's link phase: hints that the parse verifies) may produce different but equally valid output.
 // Atomics are plain read-modify-writes (one OS thread).  Exited threads count as arrived, as on the device.
+//
+// The launchers of the kernel sources compile here as they are: ZB_LAUNCH (zb_common.cuh) becomes simt::launch, and the
+// few runtime calls they make are the synchronous definitions at the end of this file.
 #pragma once
+#include <cuda_runtime.h>
 #include <ucontext.h>
 #include <cstdint>
 #include <cstdio>
@@ -70,6 +74,10 @@ static void trampoline() { g_body(); g_threads[g_cur].done = true; swapcontext(&
 static void launch(unsigned grid, unsigned block, std::function<void()> body)
 {
     size_t const STACK = 256 << 10;
+    static std::vector<char*> stacks;                           // fiber stacks, reused by every CTA of every launch
+    while (stacks.size() < block) stacks.push_back((char*)malloc(STACK));
+    static ucontext_t proto; static bool have_proto = false;     // every fiber starts from the same saved context
+    if (!have_proto) { getcontext(&proto); have_proto = true; }
     g_body = body; g_gridDim.x = grid; g_blockDim.x = block;
     for (unsigned b = 0; b < grid; b++) {
         g_blockIdx.x = b;
@@ -77,8 +85,8 @@ static void launch(unsigned grid, unsigned block, std::function<void()> body)
         g_cta_gen = 0; g_cta_arrived = 0;
         for (int q = 0; q < 16; q++) { g_nb_gen[q] = 0; g_nb_arrived[q] = 0; }
         for (unsigned t = 0; t < block; t++) {
-            Thread& T = g_threads[t]; T.stack = (char*)malloc(STACK);
-            getcontext(&T.ctx); T.ctx.uc_stack.ss_sp = T.stack; T.ctx.uc_stack.ss_size = STACK; T.ctx.uc_link = &g_sched;
+            Thread& T = g_threads[t]; T.stack = stacks[t];
+            T.ctx = proto; T.ctx.uc_stack.ss_sp = T.stack; T.ctx.uc_stack.ss_size = STACK; T.ctx.uc_link = &g_sched;
             makecontext(&T.ctx, trampoline, 0);
         }
         unsigned live = block;
@@ -108,7 +116,6 @@ static void launch(unsigned grid, unsigned block, std::function<void()> body)
                 for (size_t w = 0; w < g_warps.size(); w++) fprintf(stderr, " | warp %zu gen %u arrived %08x read %08x", w, g_warps[w].gen, g_warps[w].arrived, g_warps[w].read);
                 fprintf(stderr, " | cta gen %u arrived %u\n", g_cta_gen, g_cta_arrived); abort(); } } else idle_rounds = 0;
         }
-        for (auto& T : g_threads) free(T.stack);
     }
 }
 
@@ -215,7 +222,23 @@ static inline void __threadfence() {}
 static inline void __threadfence_block() {}
 static inline long long clock64() { return 0; }
 #define __log2f log2f
+// the bit reader's funnel shifts (PTX shf.{l,r}.{wrap,clamp}) and the other integer intrinsics
+static inline unsigned __funnelshift_r(unsigned lo, unsigned hi, unsigned s) { unsigned long long v = ((unsigned long long)hi << 32) | lo; return (unsigned)(v >> (s & 31)); }
+static inline unsigned __funnelshift_rc(unsigned lo, unsigned hi, unsigned s) { unsigned long long v = ((unsigned long long)hi << 32) | lo; s = s > 32 ? 32 : s; return (unsigned)(s == 32 ? v >> 32 : v >> s); }
+static inline unsigned __funnelshift_lc(unsigned lo, unsigned hi, unsigned s) { unsigned long long v = ((unsigned long long)hi << 32) | lo; s = s > 32 ? 32 : s; return (unsigned)((s == 32 ? (v << 31) << 1 : v << s) >> 32); }
+static inline int __clz(int v) { return v ? __builtin_clz((unsigned)v) : 32; }
+static inline int __ffs(int v) { return __builtin_ffs(v); }
+static inline int __popc(unsigned v) { return __builtin_popcount(v); }
+template <class T> static inline T __ldcg(const T* p) { return *p; }
 
 // min / max over mixed integer types, as the CUDA headers provide
 template <class A, class B> static inline typename std::common_type<A, B>::type min(A a, B b) { typedef typename std::common_type<A, B>::type T; return (T)a < (T)b ? (T)a : (T)b; }
 template <class A, class B> static inline typename std::common_type<A, B>::type max(A a, B b) { typedef typename std::common_type<A, B>::type T; return (T)a > (T)b ? (T)a : (T)b; }
+
+// a CTA's dynamic shared memory (ZB_DYN_SMEM): one CTA runs at a time
+alignas(16) static unsigned char simt_dyn_smem[256 << 10];
+
+// the runtime calls of the launchers: the CPU build does not link libcudart, and every launch has finished when it returns
+extern "C" cudaError_t cudaMemsetAsync(void* p, int v, size_t n, cudaStream_t) { memset(p, v, n); return cudaSuccess; }
+extern "C" cudaError_t cudaMemcpyAsync(void* d, const void* s, size_t n, cudaMemcpyKind, cudaStream_t) { memcpy(d, s, n); return cudaSuccess; }
+extern "C" cudaError_t cudaStreamSynchronize(cudaStream_t) { return cudaSuccess; }

@@ -18,18 +18,19 @@ import chain_encode_sim as E  # noqa: E402
 import chain_ref as R          # noqa: E402
 import chain_sim as S          # noqa: E402
 import corpus                  # noqa: E402
+import host_encoder            # noqa: E402
 
 pytestmark = pytest.mark.skipif(not os.path.exists(R.REF), reason="oracle/_ref/libzstd_ref.so not built")
 
 
 @pytest.fixture(scope="module")
 def enc():
-    return E.build()
+    return host_encoder.build_sim()
 
 
 @pytest.fixture(scope="module")
 def dec():
-    return S.build()
+    return host_encoder.build_sim()
 
 
 def text(n, off=0):

@@ -1,9 +1,9 @@
 """The compression kernels' own source, run on the CPU.
 
-tests/host_encoder.build_compress_sim() compiles python_zstandard_b200/csrc/zb_encode.cu (everything above its
-launchers: the block kernel with all its phases, the frame layout kernels, XXH64) with g++ on the mini SIMT runtime of
-tests/simt.h -- every thread of a CTA is a fiber, __syncthreads and the warp collectives are rendezvous points -- and
-drives it the way zb_api.cu does (block jobs, persistent CTAs, slots, frame sizes, scan, frame writer).  The frames go
+tests/host_encoder.build_sim() compiles python_zstandard_b200/csrc/zb_encode.cu (the block kernel with all its phases,
+the frame layout kernels, XXH64, and their launchers) with g++ on the mini SIMT runtime of tests/simt.h -- every thread
+of a CTA is a fiber, __syncthreads and the warp collectives are rendezvous points -- and calls the launchers the way
+zb_api.cu does (block jobs, persistent CTAs, slots, frame sizes, scan, frame writer).  The frames go
 through the unmodified reference decoder and the oracle.  The device build differs only in timing, so the compressed
 bytes are the same except where the link phase lets lanes of one step race for a hash slot (the hardware picks a winner
 we cannot predict); sizes are asserted against the reference with the margins the GPU suite uses."""
@@ -22,7 +22,7 @@ pytestmark = pytest.mark.skipif(not os.path.exists(REF), reason="oracle/_ref is 
 
 @pytest.fixture(scope="module")
 def sim():
-    return host_encoder.build_compress_sim()
+    return host_encoder.build_sim()
 
 
 @pytest.fixture(scope="module")

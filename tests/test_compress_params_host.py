@@ -30,7 +30,7 @@ GUARD = 1 << 16                 # bytes of input memory in front of the first se
 
 @pytest.fixture(scope="module")
 def sim():
-    return host_encoder.build_compress_sim()
+    return host_encoder.build_sim()
 
 
 @pytest.fixture(scope="module")

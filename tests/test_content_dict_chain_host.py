@@ -16,13 +16,14 @@ import chain_ref as R          # noqa: E402
 import chain_sim as S          # noqa: E402
 import corpus                  # noqa: E402
 import frame_writer as fw      # noqa: E402
+import host_encoder            # noqa: E402
 
 pytestmark = pytest.mark.skipif(not os.path.exists(R.REF), reason="oracle/_ref/libzstd_ref.so not built")
 
 
 @pytest.fixture(scope="module")
 def sim():
-    return S.build()
+    return host_encoder.build_sim()
 
 
 def one_run(k, sizes):

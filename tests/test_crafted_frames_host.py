@@ -46,7 +46,7 @@ def kern():
 
 @pytest.fixture(scope="module")
 def dsim():
-    L = host_encoder.build_decode_sim()
+    L = host_encoder.build_sim()
     yield L
     L.t_set_block_path(0)
 

@@ -5,7 +5,7 @@ overlaps the kernels of chunk k + 1.  The cuts are by frame count; every chunk h
 launch shape (warps per CTA, frames per warp, CTAs) from its own average output size, its own execute range -- frames,
 blocks or output bytes -- and its own checksum pass (zb_chunk_count, zb_chunk_cut, zb_chunk_shape in zb_common.cuh).
 
-tests/host_encoder.build_decode_sim() runs the same plan chunk by chunk on the CPU build of the kernels (`chunk_bytes`
+tests/host_encoder.build_sim() runs the same plan chunk by chunk on the CPU build of the kernels (`chunk_bytes`
 stands for ZB200_OUT_CHUNK_BYTES).  It copies each chunk's output range out as soon as the chunk's kernels are done, and
 assembles the result from those copies alone; then it overwrites the range in its working buffer, so any later write
 there -- even of the right bytes -- is counted.  Every test runs on the three execute paths, and checks the bytes against
@@ -28,7 +28,7 @@ SMS = 1          # the SM count the plan shapes the entropy launches for: 1 CTA 
 
 @pytest.fixture(scope="module", params=["lane-per-frame", "lane-per-block", "lane-per-block+pointer-jumping"])
 def sim(request):
-    L = host_encoder.build_decode_sim()
+    L = host_encoder.build_sim()
     L.t_set_block_path({"lane-per-frame": 0, "lane-per-block": 1}.get(request.param, 2))
     L.path = request.param
     yield L

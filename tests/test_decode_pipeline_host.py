@@ -1,8 +1,8 @@
 """All decompression kernels, run on the CPU kernel by kernel the way zb_api.cu launches them.
 
-tests/host_encoder.build_decode_sim() compiles zb_decode.cu + zb_entropy.cuh (frame scan, placement scans, the
+tests/host_encoder.build_sim() compiles zb_decode.cu + zb_entropy.cuh (frame scan, placement scans, the
 lane-per-frame entropy kernel with its shared-memory pool claims, both execute kernels with their dependency frontier,
-checksum verification, finish) on the mini SIMT runtime of tests/simt.h: 32 lanes per warp in lock step at every
+checksum verification, finish, and their launchers) on the mini SIMT runtime of tests/simt.h: 32 lanes per warp in lock step at every
 collective, 7 or 8 warps per CTA, persistent CTAs pulling frames from the work counter.  Output must equal the
 reference's, per-frame status codes must match what the GPU suite expects."""
 import ctypes as C
@@ -23,7 +23,7 @@ PAD = 64
 def sim(request):
     """Every test runs twice: through zb_entropy_decode (a lane per frame) and through the block-parallel path
     (zb_scan_blocks -> zb_entropy_blocks -> zb_resolve_blocks -> zb_patch_blocks: a lane per block, symbolic repcodes)."""
-    L = host_encoder.build_decode_sim()
+    L = host_encoder.build_sim()
     L.t_set_block_path({"lane-per-frame": 0, "lane-per-block": 1}.get(request.param, 2))
     yield L
     L.t_set_block_path(0)
@@ -110,8 +110,7 @@ def test_dictionary_records(sim, ref):
 def test_kernel_to_kernel_round_trip():
     """Frames written by the compression kernels (CPU build) regenerate through the decompression kernels (CPU build)."""
     from tests.test_compress_kernel_host import compress
-    csim = host_encoder.build_compress_sim()
-    dsim = host_encoder.build_decode_sim()
+    csim = dsim = host_encoder.build_sim()
     text = corpus.text_corpus(1 << 20)
     segs = [bytes(text[i * 5000:i * 5000 + 3000 + 97 * i]) for i in range(20)] + [bytes(text[200000:200000 + 140000]), bytes(5000), b"q"]
     frames = compress(csim, segs, checksum=True, n_ctas=3)

@@ -1,5 +1,5 @@
 """zb_execute_tile (frames up to 4 KiB, regenerated in a shared-memory tile with their literals staged in place at the
-tile's end) on the CPU build of the kernels (tests/host_encoder.build_decode_sim, lane-per-frame path).
+tile's end) on the CPU build of the kernels (tests/host_encoder.build_sim, lane-per-frame path).
 
 The frames are chosen for the in-place staging: groups whose later literal runs land on an earlier lane's staged
 literals, a compressed block without sequences that fills the frame (no margin at all), decompressed sizes larger than
@@ -22,7 +22,7 @@ pytestmark = pytest.mark.skipif(not os.path.exists(REF), reason="oracle/_ref is 
 
 @pytest.fixture(scope="module")
 def sim():
-    L = host_encoder.build_decode_sim()
+    L = host_encoder.build_sim()
     L.t_set_block_path(0)
     return L
 

@@ -17,8 +17,8 @@ pytestmark = pytest.mark.skipif(not os.path.exists(train_ref.REF), reason="oracl
 
 @pytest.fixture(scope="module")
 def sim():
-    from tests import train_sim
-    return train_sim.build()
+    from tests import host_encoder
+    return host_encoder.build_sim()
 
 
 def foo_samples():

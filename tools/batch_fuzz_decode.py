@@ -11,7 +11,7 @@ from oracle import RefZstd
 from tests import host_encoder
 from tests.test_decode_pipeline_host import decompress
 
-sim = host_encoder.build_decode_sim()
+sim = host_encoder.build_sim()
 ref = RefZstd()
 
 

@@ -10,7 +10,7 @@ from oracle import RefZstd
 from tests import host_encoder
 from tests.test_compress_kernel_host import compress
 
-sim = host_encoder.build_compress_sim()
+sim = host_encoder.build_sim()
 ref = RefZstd()
 rng = np.random.default_rng(int(os.environ.get("SEED", "1")))
 text = corpus.text_corpus(1 << 20)

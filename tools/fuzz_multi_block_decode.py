@@ -8,7 +8,7 @@ accepted when the reference rejects it, and has the reference's bytes when both 
 Round 2: N=40 SEED=11 (320 frames x 3 mappings): 160 healthy exact; damaged: 134 rejected by both, 19 accepted by both with equal
 bytes, 7 rejected by the kernels alone (the stricter Huffman check, DESIGN section 6).  ASAN build, N=20 SEED=23 and N=6 SEED=5: clean.
    ASAN=1 ASAN_OPTIONS=detect_leaks=0:detect_stack_use_after_return=0 LD_PRELOAD=$(gcc -print-file-name=libasan.so) N=10 python tools/fuzz_multi_block_decode.py"""
-import os, sys, subprocess, ctypes as C
+import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import corpus
@@ -16,14 +16,10 @@ from oracle import RefZstd
 from tests import host_encoder
 from tests.test_decode_pipeline_host import decompress
 
-sim = host_encoder.build_decode_sim()
 if os.environ.get("ASAN") == "1":
-    lib = "/tmp/libzd_sim_asan.so"
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-g", "-fsanitize=address", "-fno-omit-frame-pointer", "-shared", "-fPIC",
-                           "-I/usr/local/cuda/include", "-o", lib, os.path.join(host_encoder.BUILD, "zd_sim.cpp")])
-    proto = sim.t_decompress_batch
-    sim = C.CDLL(lib)
-    sim.t_decompress_batch.restype = proto.restype; sim.t_decompress_batch.argtypes = proto.argtypes
+    sim = host_encoder.build_sim("/tmp/libzsim_asan.so", ["-O1", "-g", "-fsanitize=address", "-fno-omit-frame-pointer"])
+else:
+    sim = host_encoder.build_sim()
 ref = RefZstd()
 rng = np.random.default_rng(int(os.environ.get("SEED", "1")))
 text = corpus.text_corpus(4 << 20)

@@ -2,8 +2,9 @@
 //
 // zb_decode.cu and zb_encode.cu (with zb_encode2.cuh, zb_encode3.cuh and zb_train.cuh) compile here as they are, launchers
 // included, on the SIMT runtime of simt.h; tests/host_encoder.py builds this file with ZB_SIMT_EMULATION.  The wrappers
-// below call the launchers in the order zb_api.cu calls them and plan with the host functions of zb_common.cuh, on the SM
-// counts, warps and frames per warp that the tests choose.  The CPU suite loads them over ctypes.
+// below call the kernels' serial helpers by name, and call the launchers in the order zb_api.cu calls them and plan with the
+// host functions of zb_common.cuh, on the SM counts, warps and frames per warp that the tests choose.  The CPU suite loads
+// them over ctypes; it has no other build of the kernel source.
 #include "simt.h"
 #include "zb_decode.cu"
 #include "zb_encode.cu"
@@ -50,9 +51,105 @@ struct TScan {
         zb_launch_place(info.data(), dst_sizes, n, place.data(), totals, status.data(), partial.data(), 0);
     }
 };
+
+// the decode kernels' view of a dictionary: zb_launch_digest_dict into dg, and dict pointing into it (empty without a
+// dictionary).  Returns the digest's status.
+u32 t_dict_dev(const u8* dict_raw, u32 dict_n, ZbDictDigest& dg, ZbDictDev& dict)
+{
+    memset(&dict, 0, sizeof dict);
+    if (!dict_raw || !dict_n) return ZB_OK;
+    zb_launch_digest_dict(dict_raw, dict_n, &dg, 0);
+    if (dg.status != ZB_OK) return dg.status;
+    if (dg.has_entropy) {
+        dict.content = dict_raw + dg.content_off; dict.content_size = dict_n - dg.content_off; dict.dict_id = dg.dict_id; dict.has_entropy = 1;
+        dict.huf = dg.huf; dict.huf_log = dg.huf_log; dict.ll = dg.ll; dict.of = dg.of; dict.ml = dg.ml;
+        dict.ll_log = dg.ll_log; dict.of_log = dg.of_log; dict.ml_log = dg.ml_log;
+        dict.rep[0] = dg.rep[0]; dict.rep[1] = dg.rep[1]; dict.rep[2] = dg.rep[2];
+    } else { dict.content = dict_raw; dict.content_size = dict_n; }
+    return ZB_OK;
+}
 }  // namespace
 
 extern "C" unsigned long long t_any_calls(int reset) { unsigned long long v = simt_any_calls; if (reset) simt_any_calls = 0; return v; }
+
+// ---- the serial helpers of the kernels: entropy tables, headers, literals.  None of them reaches a warp collective, a
+// barrier or shared state, so they are called directly, outside any launch.
+extern "C" {
+// encoder (zb_encode.cu)
+int t_normalize(short* norm, const u32* count, u32 max_sym, u32 total, u32 log) { return ze_normalize(norm, count, max_sym, total, log) ? 1 : 0; }
+u32 t_write_ncount(u8* out, const short* norm, u32 max_sym, u32 log) { return ze_write_ncount(out, norm, max_sym, log); }
+u32 t_cost(const u32* count, const short* norm, u32 max_sym, u32 log) { return ze_cost(count, norm, max_sym, log); }
+void t_build_ctable(const short* norm, u32 max_sym, u32 log, u16* state, int* dnb, int* dfs)
+{
+    static ZeCTable ct; static u8 tmp[512];
+    ze_build_ctable(ct, norm, max_sym, log, tmp);
+    memcpy(state, ct.state, sizeof(u16) << log); memcpy(dnb, ct.dnb, sizeof(int) * (max_sym + 1)); memcpy(dfs, ct.dfs, sizeof(int) * (max_sym + 1));
+}
+// mode, log, header bytes of the table the encoder would pick for this histogram (no dictionary)
+void t_make_table(const u32* count, u32 max_sym_kind, u32 nseq, u32 max_log, u32 def_log, const short* defnorm, u32 def_max,
+                  u32* mode, u32* log, u32* hdr_bytes, u8* hdr)
+{
+    static ZeCTable ct; static u8 tmp[512];
+    ze_make_table(ct, count, max_sym_kind, nseq, max_log, def_log, defnorm, def_max, tmp);
+    *mode = ct.mode; *log = ct.log; *hdr_bytes = ct.hdr_bytes; memcpy(hdr, ct.hdr, 64);
+}
+int t_huf_build(const u32* count, u8* nb, u16* code, u32* max_sym, u32* log)
+{
+    static ZeHuf H; static u32 wk[1600];
+    if (!ze_huf_build(H, count, wk)) return 0;
+    memcpy(nb, H.nb, 256); memcpy(code, H.code, 512); *max_sym = H.max_sym; *log = H.log;
+    return 1;
+}
+u32 t_huf_write_table(const u32* count, u8* out)
+{
+    static ZeHuf H; static u32 wk[1600]; static ZeCTable ct; static u8 tmp[512];
+    if (!ze_huf_build(H, count, wk)) return 0;
+    return ze_huf_write_table(out, H, ct, tmp);
+}
+u32 t_frame_header(u8* o, u64 size, u32 checksum, u32 content_size, u32 dict_id)
+{
+    ZeParams P; P.checksum = checksum; P.content_size = content_size; P.dict_id = dict_id; P.level = 3;
+    return ze_frame_header(o, size, P);
+}
+
+// decoder (zb_decode.cu, zb_entropy.cuh)
+// builds the split table for the given nibble weights and returns its shape; cells must hold 4096 entries
+void t_huf_split(const u8* ws, u32 log, u32 nsym, const u32* rank, u16* cells, u32* shift, u32* T, u32* base, u32* bytes)
+{
+    zb_huf_shape(log, rank, *shift, *T, *base, *bytes);
+    zb_huf_fill(cells, ws, log, nsym, rank, *shift, *base);
+}
+void t_huf_full(const u8* ws, u32 log, u32 nsym, const u32* rank, u16* cells) { zb_huf_fill(cells, ws, log, nsym, rank, 0, 0); }
+u32 t_huf_cell(const u16* cells, u32 log, u32 shift, u32 T, u32 base, u32 v)
+{
+    ZbHufTab t; t.cells = cells; t.log = log; t.shift = shift; t.T = T; t.base = base;
+    return ZB_HCELL(t, v);
+}
+// out[6] = {content_size, window, dict_id, hdr_size, checksum, status}
+void t_parse_header(const u8* s, u64 n, u64* out)
+{
+    ZbHdr h; zb_parse_header(s, n, h);
+    out[0] = h.content_size; out[1] = h.window; out[2] = h.dict_id; out[3] = h.hdr_size; out[4] = h.checksum; out[5] = h.status;
+}
+// a Huffman-coded literals payload (weights header + 1 or 4 streams, as HUF_compress{1,4}X writes it) -> regen bytes.
+// returns 1 on success, 0 on a rejected payload; *hdr_used = bytes of the weights header
+int t_literals_decode(u8* dst, u32 regen, const u8* payload, u32 n, int single, u32* hdr_used, u32* table_bytes)
+{
+    static u8 ws[256]; static u16 cells[4096 + 8]; u32 rank[13], log = 0, nsym = 0;
+    u32 const used = zb_huf_weights(ws, payload, n, log, nsym, rank);
+    *hdr_used = used;
+    if (used == 0 || used >= n) return 0;
+    u32 shift, T, base, bytes;
+    zb_huf_shape(log, rank, shift, T, base, bytes);
+    *table_bytes = bytes;
+    zb_huf_fill(cells, ws, log, nsym, rank, shift, base);
+    ZbHufTab t; t.cells = cells; t.log = log; t.shift = shift; t.T = T; t.base = base;
+    return zb_huf_block(dst, regen, payload + used, n - used, single != 0, t) ? 1 : 0;
+}
+// the tANS decode table of one sequence stream (kind 0 LL, 1 OF, 2 ML): cells[1 << log], norm is consumed
+void t_build_fse(u32* cells, short* norm, u32 max_sym, u32 log, int kind) { zb_build_fse((ZbFseCell*)cells, norm, max_sym, log, kind); }
+u32 t_read_ncount(short* norm, u32* max_sym, u32* log, const u8* s, u32 n) { u32 ms = *max_sym, lg = 0; u32 r = zb_read_ncount(norm, ms, lg, s, n); *max_sym = ms; *log = lg; return r; }
+}
 
 // ---- compression
 // The whole compression path of the library: block jobs cut as zb_api.cu cuts them (zb_cut_blocks, blocks of
@@ -151,6 +248,61 @@ extern "C" void t_scan_totals(const u8* src, const u64* seg_off, const u64* seg_
     for (int k = 0; k < 6; k++) totals_out[k] = S.totals[k];
 }
 
+// Decode ONE frame through the launchers, as the library runs a batch of one: default tables, dictionary digest, scan,
+// placement, then the lane-per-frame entropy kernel on one CTA of 7 warps with one frame per warp.  The output capacity is
+// the frame's content size, or `cap` when the header does not state one.  The bytes are then regenerated from the kernel's
+// block / sequence / literal records by a serial replay that shares no code with the execute kernels.  Returns the status
+// code; *out_n = bytes produced.
+extern "C" int t_decode_frame(const u8* src, u64 n, const u8* dict_raw, u32 dict_n, u8* out, u64 cap, u64* out_n, u32* n_blocks, u32* n_seq)
+{
+    static bool tables = false;
+    if (!tables) { zb_launch_default_tables(0); tables = true; }
+    static ZbDictDigest dg; ZbDictDev dict;
+    if (u32 const st = t_dict_dev(dict_raw, dict_n, dg, dict)) return (int)st;
+    ZbSegment seg; seg.offset = 0; seg.length = n;
+    ZbFrameInfo fi; u32 big[2];
+    zb_launch_scan(src, &seg, 1, &fi, (1ull << 27) + 1, big, 0);
+    if (fi.status != ZB_OK) return (int)fi.status;
+    u64 const want = fi.content_size != ZB_CONTENT_UNKNOWN ? fi.content_size : cap;
+    if (want > cap) return (int)ZB_E_DSTSIZE_TOO_SMALL;
+    ZbFramePlace place[2]; u64 totals[8] = {0}, partial[8]; u32 status = ZB_OK;
+    zb_launch_place(&fi, &want, 1, place, totals, &status, partial, 0);
+    std::vector<ZbBlock> vblocks(fi.n_blocks + 1); std::vector<ZbSeq> vseqs(fi.n_seq_rec + 2); std::vector<u8> vlits(fi.n_lit + 64);
+    ZbBlock* const blocks = vblocks.data(); ZbSeq* const seqs = vseqs.data(); u8* const lits = vlits.data();
+    u32 counter = 0, ck = 0; u64 out_size = 0;
+    zb_launch_entropy(src, &seg, 1, place, fi.content_size != ZB_CONTENT_UNKNOWN ? &want : nullptr, blocks, seqs, lits, 1, &counter, dict, &status,
+                      &out_size, &ck, 1, 7, 0);
+    *n_blocks = fi.n_blocks; *n_seq = 0;
+    // zb_finish's job for one frame; the kernel records errors in status[]
+    int rc = (int)status;
+    if (rc == ZB_OK) {
+        const u8* const dict_end = dict.content + dict.content_size;
+        u64 total = 0;
+        for (u32 bi = 0; bi < fi.n_blocks; bi++) {
+            ZbBlock const& B = blocks[bi];
+            u8* const bout = out + B.out_pos;
+            if (B.out_pos + B.regen > cap) { rc = (int)ZB_E_DSTSIZE_TOO_SMALL; break; }
+            if (B.kind == ZB_BLK_RAW) memcpy(bout, src + B.src_pos, B.regen);
+            else if (B.kind == ZB_BLK_RLE) memset(bout, (int)B.lit_byte, B.regen);
+            else {
+                const u8* const lit = B.lit_kind == ZB_LIT_RAW ? src + B.src_pos : lits + B.src_pos;
+                const ZbSeq* const sq = seqs + B.seq_pos;
+                *n_seq += B.n_seq;
+                for (u32 i = 0; i <= B.n_seq; i++) {
+                    u32 const ll = i < B.n_seq ? sq[i + 1].x - sq[i].x : B.n_lit - sq[i].x;
+                    for (u32 k = 0; k < ll; k++) bout[sq[i].y + k] = B.lit_kind == ZB_LIT_RLE ? (u8)B.lit_byte : lit[sq[i].x + k];
+                    if (i == B.n_seq) break;
+                    long long const m0 = (long long)B.out_pos + sq[i].y + ll;
+                    for (u32 k = 0; k < sq[i].z; k++) { long long const sp = m0 + k - (long long)sq[i].w; out[m0 + k] = sp < 0 ? dict_end[sp] : out[sp]; }
+                }
+            }
+            total = B.out_pos + B.regen;
+        }
+        *out_n = total;
+    }
+    return rc;
+}
+
 // The whole decompression path (run_decompress): scan, placement, the entropy stage -- a lane per frame on `n_ctas` CTAs of
 // `warps` warps with `take` frames per warp, or a lane per block (t_set_block_path 1: execute by zb_execute_big, 2: by
 // pointer jumping) -- execute, checksums, finish.  Output: tightly packed bytes + per-frame {offset, length}, status[] per
@@ -174,17 +326,8 @@ extern "C" long long t_decompress_batch(const u8* src, const u64* seg_off, const
 {
     static bool tables = false;
     if (!tables) { zb_launch_default_tables(0); tables = true; }
-    static ZbDictDigest dg; ZbDictDev dict; memset(&dict, 0, sizeof dict);
-    if (dict_raw && dict_n) {
-        zb_launch_digest_dict(dict_raw, dict_n, &dg, 0);
-        if (dg.status != ZB_OK) return -(long long)dg.status;
-        if (dg.has_entropy) {
-            dict.content = dict_raw + dg.content_off; dict.content_size = dict_n - dg.content_off; dict.dict_id = dg.dict_id; dict.has_entropy = 1;
-            dict.huf = dg.huf; dict.huf_log = dg.huf_log; dict.ll = dg.ll; dict.of = dg.of; dict.ml = dg.ml;
-            dict.ll_log = dg.ll_log; dict.of_log = dg.of_log; dict.ml_log = dg.ml_log;
-            dict.rep[0] = dg.rep[0]; dict.rep[1] = dg.rep[1]; dict.rep[2] = dg.rep[2];
-        } else { dict.content = dict_raw; dict.content_size = dict_n; }
-    }
+    static ZbDictDigest dg; ZbDictDev dict;
+    if (u32 const st = t_dict_dev(dict_raw, dict_n, dg, dict)) return -(long long)st;
     TScan S(src, seg_off, seg_len, n, dst_sizes);
     ZbFramePlace* const place = S.place.data(); u32* const status = S.status.data(); u64 const* const totals = S.totals;
     if (totals[0] > out_cap) return -1000;

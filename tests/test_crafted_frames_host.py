@@ -40,11 +40,6 @@ def orc():
 
 
 @pytest.fixture(scope="module")
-def kern():
-    return host_encoder.build_entropy_kernel()
-
-
-@pytest.fixture(scope="module")
 def dsim():
     L = host_encoder.build_sim()
     yield L
@@ -98,13 +93,14 @@ def _single(kern, c):
     return rc, bytes(out[PAD:PAD + out_n.value])
 
 
-def test_one_lane(kern):
-    """The lane-per-frame kernel's code with one lane, one frame at a time.  (The content checksum is compared by
-    zb_verify_checksums, which only the batch pipeline runs: the wrong checksum is checked on every path below.)"""
+def test_one_lane(dsim):
+    """The lane-per-frame kernel through its launcher, one frame per call: one busy lane in a warp.  (The content
+    checksum is compared by zb_verify_checksums, which only the batch pipeline runs: the wrong checksum is checked on
+    every path below.)"""
     for c in CASES + DICT_REPS:
         if c.name == "wrong_checksum":
             continue
-        rc, got = _single(kern, c)
+        rc, got = _single(dsim, c)
         if c.expected is None:
             assert rc != 0, c.name
         else:

@@ -1,8 +1,8 @@
-"""CPU tests of the decoder's literal path on a host build of the kernel's own source lines (tests/host_encoder.py):
-bit reader (zb_common.cuh), NCount reader (zb_decode.cu), Huffman weights, split decode table and the 1- and
-4-stream decoders (zb_entropy.cuh) -- against payloads written by the reference's HUF_compress1X/4X
-(zstd/zstd.c:18193, :18207) and against FSE_readNCount (:3433).  The GPU parity tests cover the same code inside the
-kernel; these run everywhere and fuzz harder."""
+"""CPU tests of the decoder's literal path on the CPU build of the kernel source (tests/host_encoder.build_sim), whose
+wrappers call the helpers by name: bit reader (zb_common.cuh), NCount reader (zb_decode.cu), Huffman weights, split
+decode table and the 1- and 4-stream decoders (zb_entropy.cuh) -- against payloads written by the reference's
+HUF_compress1X/4X (zstd/zstd.c:18193, :18207) and against FSE_readNCount (:3433).  The GPU parity tests cover the same
+code inside the kernel; these run everywhere and fuzz harder."""
 import ctypes as C
 import os
 
@@ -18,7 +18,7 @@ PAD = 64
 
 @pytest.fixture(scope="module")
 def libs():
-    ours = host_encoder.build_literals_decoder()
+    ours = host_encoder.build_sim()
     ref = C.CDLL(REF)
     for name in ("HUF_compress1X_repeat", "HUF_compress4X_repeat", "FSE_normalizeCount", "FSE_writeNCount", "FSE_readNCount"):
         getattr(ref, name).restype = C.c_size_t
@@ -206,9 +206,7 @@ def test_frame_header_parser_equals_the_reference(libs):
     """The device header parser (zb_parse_header) against ZSTD_getFrameHeader (zstd/zstd.c:43668) on headers the
     reference wrote, on headers our encoder writes, and on thousands of random mutations: same accept / need-more / reject
     decision, same fields when accepted."""
-    _, ref = libs
-    P = host_encoder.build_header_parser()
-    H = host_encoder.build_frame_header()
+    ours, ref = libs
     ref.ZSTD_getFrameHeader.restype = C.c_size_t
     ref.ZSTD_isError.restype = C.c_uint
     from oracle import RefZstd
@@ -223,7 +221,7 @@ def test_frame_header_parser_equals_the_reference(libs):
     for did in (0, 9, 40000, 1123828263):
         for cs in (0, 1):
             out = (C.c_ubyte * 32)()
-            n = H.t_frame_header(out, 70000, 1, cs, did)
+            n = ours.t_frame_header(out, 70000, 1, cs, did)
             seeds.append(bytes(out[:n]) + bytes(18 - n))
     accepted = rejected = short = 0
     for seed in seeds:
@@ -237,7 +235,7 @@ def test_frame_header_parser_equals_the_reference(libs):
             zfh = (C.c_uint64 * 8)()
             r = ref.ZSTD_getFrameHeader(zfh, src, n)
             out = (C.c_uint64 * 6)()
-            P.t_parse_header(src, n, out)
+            ours.t_parse_header(src, n, out)
             status = out[5]
             if ref.ZSTD_isError(C.c_size_t(r)):
                 assert status != 0, (bytes(b[:n]).hex(), r)

@@ -1,8 +1,8 @@
 """CPU known-answer tests of the encoder's entropy-table code against the reference's own functions.
 
-tests/host_encoder.py compiles the serial helpers of python_zstandard_b200/csrc/zb_encode.cu (the very source lines
-the kernel runs: NCount writer, CTable builder, normalisation, table choice, Huffman code + weight header) for the
-host; oracle/_ref/libzstd_ref.so is the unmodified reference (zstd/zstd.c) and exports FSE_normalizeCount
+tests/host_encoder.build_sim() compiles python_zstandard_b200/csrc/zb_encode.cu whole for the host, and its wrappers
+call the kernel's serial helpers (NCount writer, CTable builder, normalisation, table choice, Huffman code + weight
+header) by name; oracle/_ref/libzstd_ref.so is the unmodified reference (zstd/zstd.c) and exports FSE_normalizeCount
 (:16402), FSE_writeNCount (:16267), FSE_readNCount (:3433), FSE_buildCTable_wksp (:16005), HUF_buildCTable_wksp
 (:17513) and HUF_readStats (:3448).  Bit-exact where the format leaves no freedom (NCount bytes, CTable cells,
 weight headers that decode to our code lengths); within a stated cost margin where it does (normalisation,
@@ -24,7 +24,7 @@ LL_DEF = [4, 3, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 1, 1, 1, 2, 2, 2, 2, 2, 2, 2, 2
 
 @pytest.fixture(scope="module")
 def libs():
-    ours = host_encoder.build()
+    ours = host_encoder.build_sim()
     ref = C.CDLL(REF)
     for name in ("FSE_normalizeCount", "FSE_writeNCount", "FSE_readNCount", "FSE_buildCTable_wksp", "HUF_buildCTable_wksp",
                  "HUF_readStats"):
@@ -230,7 +230,6 @@ def test_split_huffman_decode_table_equals_the_full_table(libs):
     """The decoder keeps full-resolution cells only for codes longer than 8 bits (zb_entropy.cuh).  For every code our
     encoder can emit, every index of the reference-shaped full table must read the same cell through the split table."""
     ours, ref = libs
-    dec = host_encoder.build_decoder_helpers()
     rng = np.random.default_rng(10)
     text = open(__file__, "rb").read()
     samples = [np.frombuffer(text, dtype=np.uint8), np.frombuffer(text[:900], dtype=np.uint8),
@@ -249,13 +248,13 @@ def test_split_huffman_decode_table_equals_the_full_table(libs):
             ws[s >> 1] |= w << ((s & 1) * 4)
             rank[w] += 1 if w else 0
         full = (C.c_uint16 * 4096)(); split = (C.c_uint16 * 4096)()
-        dec.t_huf_full(ws, log, nsym, rank, full)
+        ours.t_huf_full(ws, log, nsym, rank, full)
         shift, T, base, nbytes = C.c_uint32(), C.c_uint32(), C.c_uint32(), C.c_uint32()
-        dec.t_huf_split(ws, log, nsym, rank, split, C.byref(shift), C.byref(T), C.byref(base), C.byref(nbytes))
+        ours.t_huf_split(ws, log, nsym, rank, split, C.byref(shift), C.byref(T), C.byref(base), C.byref(nbytes))
         assert nbytes.value <= 2 << log and (shift.value == 0) == (log <= 8)
         saw_split |= shift.value > 0 and nbytes.value < (2 << log)
         for v in range(1 << log):
-            assert dec.t_huf_cell(split, log, shift.value, T.value, base.value, v) == full[v], (log, v)
+            assert ours.t_huf_cell(split, log, shift.value, T.value, base.value, v) == full[v], (log, v)
         # and the full table is the canonical one: index -> (symbol, length) of the code that prefixes it
         for s in range(nsym):
             if nb[s]:
@@ -270,7 +269,7 @@ def test_frame_header_bytes_equal_the_reference():
     reference parses back when the content size is left out."""
     from oracle import RefZstd
     ref = RefZstd()
-    H = host_encoder.build_frame_header()
+    H = host_encoder.build_sim()
     rng = np.random.default_rng(11)
     for size in (0, 1, 255, 256, 257, 4096, 65791, 65792, 131072, 300000, 1 << 20, 2 << 20, (2 << 20) + 1, 3 << 20, 9 << 20):
         data = rng.integers(0, 256, size).astype(np.uint8).tobytes() if size <= (1 << 20) else bytes(size)

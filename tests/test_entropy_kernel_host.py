@@ -1,11 +1,13 @@
 """The decode kernels' own source, run on the CPU.
 
-tests/host_encoder.build_entropy_kernel() compiles python_zstandard_b200/csrc/zb_decode.cu (frame scan, dictionary
-digest) and zb_entropy.cuh (the whole lane-per-frame entropy kernel: block loop, literal sections, sequence headers,
-table builds, the 3-state sequence stream, repcode history, every validity check) with g++ and stand-ins for the warp
-primitives that see one lane.  A frame goes through the kernel code, a serial loop replays the block / sequence /
-literal records the way the execute kernels read them, and the bytes must equal the reference's.  What this cannot show
-is the interplay of 32 lanes (pool claims, second passes) and the execute kernels themselves -- the GPU suite does."""
+tests/host_encoder.build_sim() compiles python_zstandard_b200/csrc/zb_decode.cu and zb_entropy.cuh whole on the SIMT
+runtime of tests/simt.h.  t_decode_frame runs a frame through the launchers as the library runs a batch of one: dictionary
+digest, frame scan, placement, and the whole lane-per-frame entropy kernel (block loop, literal sections, sequence headers,
+table builds, the 3-state sequence stream, repcode history, every validity check) on one CTA of 7 warps, with the warp
+collectives of the device.  A serial loop replays the block / sequence / literal records the way the execute kernels read
+them, and the bytes must equal the reference's.  With one frame per call the other 31 lanes of its warp are idle: the
+interplay of busy lanes (pool claims, second passes) and the execute kernels themselves are covered by the batch tests
+(test_decode_pipeline_host.py, test_crafted_frames_host.py) and the GPU suite."""
 import ctypes as C
 import os
 
@@ -21,7 +23,7 @@ PAD = 64
 
 @pytest.fixture(scope="module")
 def kern():
-    return host_encoder.build_entropy_kernel()
+    return host_encoder.build_sim()
 
 
 def decode(kern, frame, cap, dct=b""):

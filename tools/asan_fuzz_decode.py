@@ -1,18 +1,16 @@
-"""AddressSanitizer fuzz of the decode kernels' source on the CPU (tests/host_encoder.build_entropy_kernel, one emulated
-lane): mutated and truncated golden frames in exact-size heap blocks with PAD bytes of slack on both sides.
-  ASAN_OPTIONS=detect_leaks=0 LD_PRELOAD=$(gcc -print-file-name=libasan.so) N=1500 SEED=7 python tools/asan_fuzz_decode.py
+"""AddressSanitizer fuzz of the decode kernels' source on the CPU (t_decode_frame of tests/host_encoder.build_sim: one
+frame through the launchers and the lane-per-frame entropy kernel): mutated and truncated golden frames in exact-size heap
+blocks with PAD bytes of slack on both sides.
+  ASAN_OPTIONS=detect_leaks=0 LD_PRELOAD=$(gcc -print-file-name=libasan.so) N=50 SEED=1 python tools/asan_fuzz_decode.py
 The default PAD=16 covers the bit reader's by-design reads: it copies the 16-byte aligned chunks that cover a stream (up to 15
-bytes past the segment, inside its allocation granule on the device); smaller PADs show those reads."""
-import sys, os, ctypes as C, numpy as np, subprocess
+bytes past the segment, inside its allocation granule on the device); smaller PADs show those reads.
+The kernels run on simt.h's ucontext fibers, which ASan supports only in part (it warns about makecontext / swapcontext):
+check a report against the fiber stacks first.  N=50 SEED=1: 800 fuzzed, 230 accepted, no report (~8 minutes once
+built)."""
+import sys, os, ctypes as C, numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from tests import helpers, host_encoder
-# build ASAN variant of the kernel lib
-cpp=os.path.join(host_encoder.BUILD,'zk_host.cpp')
-host_encoder.build_entropy_kernel()
-lib='/tmp/libzk_asan.so'
-subprocess.check_call(['g++','-std=c++17','-O1','-g','-fsanitize=address','-fno-omit-frame-pointer','-shared','-fPIC','-I/usr/local/cuda/include','-o',lib,cpp])
-L=C.CDLL(lib)
-L.t_decode_frame.argtypes=[C.c_void_p,C.c_uint64,C.c_void_p,C.c_uint32,C.c_void_p,C.c_uint64,C.POINTER(C.c_uint64),C.POINTER(C.c_uint32),C.POINTER(C.c_uint32)]
+L=host_encoder.build_sim("/tmp/libzsim_asan.so", ["-O1", "-g", "-fsanitize=address", "-fno-omit-frame-pointer"])
 PAD=int(os.environ.get('PAD','16'))
 libc=C.CDLL(None); libc.malloc.restype=C.c_void_p; libc.malloc.argtypes=[C.c_size_t]; libc.free.argtypes=[C.c_void_p]
 def decode(frame,cap,dct=b''):

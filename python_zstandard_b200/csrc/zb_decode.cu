@@ -429,11 +429,13 @@ __device__ __forceinline__ u32 zb_code_add_bits(u32 sym, int kind)
     return kind == K_LL ? c_LL_bits[sym] : (kind == K_ML ? c_ML_bits[sym] : sym);
 }
 
-// tANS decode table (restates ZSTD_buildFSETable_body, zstd/zstd.c:46118-46233), serial.
-// `norm` (max_sym + 1 shorts) is consumed: it becomes the per-symbol next-state counters in place.
-// Cells: 32-bit ZbFseCell, or the entropy kernels' 16-bit ZB_CELL16.
-template <typename Cell = ZbFseCell>
-__device__ static void zb_build_fse(Cell* t, short* norm, u32 max_sym, u32 log, int kind)
+// Symbol spread of a tANS decode table (ZSTD_buildFSETable_body, zstd/zstd.c:46118-46233): t[u] = the symbol of cell u.
+// `norm` (max_sym + 1 shorts) becomes each symbol's first next-state counter: its count, or 1 for a -1 ("less than one")
+// symbol, which takes one cell at the top.  The placement steps past those top cells; without -1 symbols it steps once per
+// cell.  (A copy of the placement loop for that case, without the walk, made the lane-per-block entropy kernel 3 % slower
+// on 128 KiB blocks and saved nothing measurable, so there is one loop.)
+template <typename Cell>
+__device__ __forceinline__ void zb_fse_spread(Cell* t, short* norm, u32 max_sym, u32 log)
 {
     u32 const size = 1u << log, mask = size - 1, step = (size >> 1) + (size >> 3) + 3;
     u32 high = size - 1;
@@ -444,6 +446,16 @@ __device__ static void zb_build_fse(Cell* t, short* norm, u32 max_sym, u32 log, 
         if (c & 0x4000) { norm[s] = 1; continue; }
         for (int i = 0; i < c; i++) { t[pos] = (Cell)s; do pos = (pos + step) & mask; while (pos > high); }
     }
+}
+
+// tANS decode table (restates ZSTD_buildFSETable_body, zstd/zstd.c:46118-46233), serial: the spread, then every cell's
+// state from its symbol's counter in index order.  `norm` (max_sym + 1 shorts) is consumed: it becomes those counters.
+// Cells: 32-bit ZbFseCell, or the entropy kernels' 16-bit ZB_CELL16.
+template <typename Cell = ZbFseCell>
+__device__ static void zb_build_fse(Cell* t, short* norm, u32 max_sym, u32 log, int kind)
+{
+    zb_fse_spread(t, norm, max_sym, log);
+    u32 const size = 1u << log;
     for (u32 u = 0; u < size; u++) {
         u32 const s = t[u], x = (u32)(u16)norm[s]; norm[s] = (short)(x + 1);
         u32 const nb = log - (u32)zb_hibit(x);
@@ -1675,7 +1687,7 @@ __global__ void zb_digest_dict(const u8* __restrict__ dict, u32 n, ZbDictDigest*
     out->dict_id = zb_rd32(dict + 4);
     const u8* p = dict + 8; const u8* const end = dict + n;
     {
-        __align__(16) u8 ws[256]; u32 rank[13], log, nsym;
+        __align__(16) u8 ws[256]; ZbRank rank; u32 log, nsym;
 #ifdef __CUDA_ARCH__
         __shared__ __align__(16) u8 ring[64];
 #else

@@ -27,6 +27,14 @@
 // all in 16-bit cells (ZB_CELL16).  So every table the sequence loop reads is in shared memory and is addressed by a
 // 32-bit offset: its cell loads are LDS.
 #define ZB_ENT_WS_BYTES   256                     // per-lane workspace (weights / normalized counts)
+// Lanes' workspaces lie 16 bytes further apart than their size.  The lanes of a warp touch the same workspace offset at the
+// same moment (norm[s] while the FSE tables are built, the nibble of weight i), and at a 256-byte stride all 32 of those
+// addresses fall in one bank; at 272 bytes they spread over 8 banks (shared memory is 32 banks of 4 bytes, and the bit
+// readers' rings need 16-byte alignment, so 8 is the most a 16-byte skew gives).  The claim of the three FSE tables and the
+// weight stream's rings are odd multiples of 16 bytes for the same reason; the Huffman table's claim is not skewed (its
+// size varies from lane to lane, and its pool space is the tighter one).
+#define ZB_ENT_WS_STRIDE  (ZB_ENT_WS_BYTES + 16)
+#define ZB_ENT_SKEW(b)    ((((b) + 15u) & ~15u) | 16u)    // a claim of b bytes, rounded up to an odd multiple of 16
 #define ZB_ENT_DEF_LL     512                     // after the baselines (LL_base, ML_base): predefined LL, OF, ML cells
 #define ZB_ENT_DEF_OF     (ZB_ENT_DEF_LL + 2 * 64)
 #define ZB_ENT_DEF_ML     (ZB_ENT_DEF_OF + 2 * 32)
@@ -59,72 +67,87 @@ __device__ __forceinline__ u32 zb_warp_incl_scan(u32 v, u32 lane)
     return v;
 }
 
+// Small counters packed into registers: field i (BITS wide) sits in word i / (32 / BITS).  Every access selects among the
+// words with constant indices, so the lane's per-weight counts and cursors need no local memory.
+template <int WORDS, int BITS>
+struct ZbPacked {
+    static constexpr u32 PER = 32 / BITS, MASK = (1u << BITS) - 1;
+    u32 w[WORDS];
+    __device__ __forceinline__ void clear() {
+        #pragma unroll
+        for (int j = 0; j < WORDS; j++) w[j] = 0;
+    }
+    __device__ __forceinline__ u32 get(u32 i) const {
+        u32 const q = i / PER; u32 v = w[0];
+        #pragma unroll
+        for (int j = 1; j < WORDS; j++) v = q == (u32)j ? w[j] : v;
+        return (v >> (BITS * (i - q * PER))) & MASK;
+    }
+    __device__ __forceinline__ void add(u32 i, u32 v) {
+        u32 const q = i / PER, d = v << (BITS * (i - q * PER));
+        #pragma unroll
+        for (int j = 0; j < WORDS; j++) w[j] += q == (u32)j ? d : 0u;
+    }
+};
+// the count of every Huffman weight 1..12 (at most 255 each), field wt - 1
+struct ZbRank : ZbPacked<4, 10> {
+    __device__ __forceinline__ u32 operator[](u32 wt) const { return get(wt - 1); }
+    __device__ __forceinline__ void count(u32 wt) { if (wt) add(wt - 1, 1); }
+};
+
 // --- Huffman weights (HUF_readStats_body).  Weights go to ws as nibbles; the weight-FSE table
 // --- (<= 64 cells, u16: sym | nb << 4 | next << 8) sits in ws + 128.
-// returns header bytes consumed (0 = error); out: log, rank[] (count of every weight)
+// returns header bytes consumed (0 = error); out: log, rank (count of every weight)
 // `ring`: 64 bytes of the lane's shared memory for the bit reader (ws is full here)
-__device__ static u32 zb_huf_weights(u8* ws, const u8* s, u32 n, u32& out_log, u32& out_nsym, u32* rank, ZB_RING_ARG(ring))
+__device__ static u32 zb_huf_weights(u8* ws, const u8* s, u32 n, u32& out_log, u32& out_nsym, ZbRank& rank, ZB_RING_ARG(ring))
 {
     u8* const wn = ws;                       // 128 bytes: 256 nibbles
     u16* const wt = (u16*)(ws + 128);        // 64 cells
     u32 nsym, hdr;
     if (n == 0) return 0;
-    #pragma unroll
-    for (int i = 0; i < 13; i++) rank[i] = 0;
-    for (int i = 0; i < 32; i++) ((u32*)wn)[i] = 0;
+    rank.clear();
     u32 total = 0;
     auto put = [&](u32 i, u32 w) { wn[i >> 1] |= (u8)(w << ((i & 1) * 4)); };
+    auto clear_nibbles = [&] { for (int i = 0; i < 32; i++) ((u32*)wn)[i] = 0; };
     if (s[0] >= 128) {
         nsym = (u32)s[0] - 127; hdr = (nsym + 1) / 2;
         if (hdr + 1 > n) return 0;
+        clear_nibbles();
         for (u32 i = 0; i < nsym; i++) {
             u32 b = s[1 + i / 2], w = (i & 1) ? (b & 15) : (b >> 4);
             if (w > 12) return 0;
-            put(i, w); rank[w]++; total += (1u << w) >> 1;
+            put(i, w); rank.count(w); total += (1u << w) >> 1;
         }
     } else {
         hdr = s[0];
         if (hdr + 1 > n) return 0;
-        // normalized counts of the weight alphabet: only symbols 0..15 can carry a count here
-        short norm[16]; u32 max_sym = 255, log;
-        {
-            short nn[256];
-            u32 used = zb_read_ncount(nn, max_sym, log, s + 1, hdr);
-            if (used == 0 || log > 6) return 0;
-            for (u32 i = 16; i <= max_sym; i++) if (nn[i]) return 0;   // a weight > 15 could never be valid
-            if (max_sym > 15) max_sym = 15;
-            for (u32 i = 0; i <= max_sym; i++) norm[i] = nn[i];
-            // spread (FSE_buildDTable_internal, zstd/zstd.c:3680)
-            u32 const size = 1u << log, mask = size - 1, step = (size >> 1) + (size >> 3) + 3;
-            u32 high = size - 1, pos = 0;
-            u8 next[16];
-            for (u32 sy = 0; sy <= max_sym; sy++) {
-                if (norm[sy] == -1) { wt[high--] = (u16)sy; next[sy] = 1; } else next[sy] = (u8)norm[sy];
-            }
-            for (u32 sy = 0; sy <= max_sym; sy++) {
-                int const c = norm[sy];
-                for (int i = 0; i < c; i++) { wt[pos] = (u16)sy; do pos = (pos + step) & mask; while (pos > high); }
-            }
-            for (u32 u = 0; u < size; u++) {
-                u32 const sy = wt[u], x = next[sy]++;
-                u32 const nb = log - (u32)zb_hibit(x);
-                wt[u] = (u16)(sy | (nb << 4) | (((x << nb) - size) << 8));
-            }
-            ZbBitR<4> b;
-            if (!b.init(s + 1 + used, hdr - used, ring)) return 0;
-            u32 s1 = b.read(log), s2 = b.read(log); b.refill();
-            if (b.left() < 0) return 0;
-            nsym = 0;
-            for (;;) {     // two interleaved states (FSE_decompress_usingDTable_generic, zstd/zstd.c:3840-3856)
-                if (nsym + 2 > 255) return 0;
-                { u32 c = wt[s1], w = c & 15; if (w > 12) return 0; put(nsym, w); rank[w]++; total += (1u << w) >> 1; nsym++;
-                  s1 = (c >> 8) + b.read((c >> 4) & 15); b.refill(); }
-                if (b.left() < 0) { u32 w = wt[s2] & 15; if (w > 12) return 0; put(nsym, w); rank[w]++; total += (1u << w) >> 1; nsym++; break; }
-                if (nsym + 2 > 255) return 0;
-                { u32 c = wt[s2], w = c & 15; if (w > 12) return 0; put(nsym, w); rank[w]++; total += (1u << w) >> 1; nsym++;
-                  s2 = (c >> 8) + b.read((c >> 4) & 15); b.refill(); }
-                if (b.left() < 0) { u32 w = wt[s1] & 15; if (w > 12) return 0; put(nsym, w); rank[w]++; total += (1u << w) >> 1; nsym++; break; }
-            }
+        // normalized counts of the weight alphabet, in the nibbles' bytes until the table is built.  A count above symbol 15
+        // could never give a valid weight, so the read stops at symbol 15 and fails when the counts go on.
+        short* const norm = (short*)wn; u32 max_sym = 15, log;
+        u32 const used = zb_read_ncount(norm, max_sym, log, s + 1, hdr);
+        if (used == 0 || log > 6) return 0;
+        zb_fse_spread(wt, norm, max_sym, log);                       // norm: now each symbol's next-state counter
+        u32 const size = 1u << log;
+        for (u32 u = 0; u < size; u++) {
+            u32 const sy = wt[u], x = (u32)(u16)norm[sy]; norm[sy] = (short)(x + 1);
+            u32 const nb = log - (u32)zb_hibit(x);
+            wt[u] = (u16)(sy | (nb << 4) | (((x << nb) - size) << 8));
+        }
+        clear_nibbles();
+        ZbBitR<4> b;
+        if (!b.init(s + 1 + used, hdr - used, ring)) return 0;
+        u32 s1 = b.read(log), s2 = b.read(log); b.refill();
+        if (b.left() < 0) return 0;
+        nsym = 0;
+        for (;;) {     // two interleaved states (FSE_decompress_usingDTable_generic, zstd/zstd.c:3840-3856)
+            if (nsym + 2 > 255) return 0;
+            { u32 c = wt[s1], w = c & 15; if (w > 12) return 0; put(nsym, w); rank.count(w); total += (1u << w) >> 1; nsym++;
+              s1 = (c >> 8) + b.read((c >> 4) & 15); b.refill(); }
+            if (b.left() < 0) { u32 w = wt[s2] & 15; if (w > 12) return 0; put(nsym, w); rank.count(w); total += (1u << w) >> 1; nsym++; break; }
+            if (nsym + 2 > 255) return 0;
+            { u32 c = wt[s2], w = c & 15; if (w > 12) return 0; put(nsym, w); rank.count(w); total += (1u << w) >> 1; nsym++;
+              s2 = (c >> 8) + b.read((c >> 4) & 15); b.refill(); }
+            if (b.left() < 0) { u32 w = wt[s1] & 15; if (w > 12) return 0; put(nsym, w); rank.count(w); total += (1u << w) >> 1; nsym++; break; }
         }
     }
     if (total == 0) return 0;
@@ -132,7 +155,7 @@ __device__ static u32 zb_huf_weights(u8* ws, const u8* s, u32 n, u32& out_log, u
     if (log > 12) return 0;
     u32 const rest = (1u << log) - total, hb = (u32)zb_hibit(rest);
     if ((1u << hb) != rest) return 0;
-    put(nsym, hb + 1); rank[hb + 1]++; nsym++;
+    put(nsym, hb + 1); rank.count(hb + 1); nsym++;
     if (rank[1] < 2 || (rank[1] & 1)) return 0;
     out_log = log; out_nsym = nsym;
     return hdr + 1;
@@ -147,23 +170,31 @@ __device__ static u32 zb_huf_weights(u8* ws, const u8* s, u32 n, u32& out_log, u
 // A 4 KiB text frame needs ~600 bytes instead of 2 KB, so all 32 lanes of a warp decode in one pass.
 #define ZB_HUF_COARSE 8u
 struct ZbHufTab { const u16* cells; u32 log, shift, T, base; };       // base = index of coarse[0] in cells
-__device__ __forceinline__ void zb_huf_shape(u32 log, const u32* rank, u32& shift, u32& T, u32& base, u32& bytes)
+__device__ __forceinline__ void zb_huf_shape(u32 log, ZbRank const& rank, u32& shift, u32& T, u32& base, u32& bytes)
 {
     shift = log > ZB_HUF_COARSE ? log - ZB_HUF_COARSE : 0u;
-    T = 0; for (u32 wt = 1; wt <= shift; wt++) T += rank[wt] << (wt - 1);
+    T = 0;
+    #pragma unroll
+    for (u32 wt = 1; wt <= 12 - ZB_HUF_COARSE; wt++) T += wt <= shift ? rank[wt] << (wt - 1) : 0u;
     base = (T + 3u) & ~3u;
     bytes = 2u * (base + (1u << (log - shift)));
 }
 __device__ __forceinline__ ZbHufTab zb_huf_full(const u16* cells, u32 log) { ZbHufTab t; t.cells = cells; t.log = log; t.shift = 0; t.T = 0; t.base = 0; return t; }
 #define ZB_HCELL(t, v) ((t).cells[(v) < (t).T ? (v) : (t).base + ((v) >> (t).shift)])
 
-// fill the decode cells (u16: symbol | nbBits << 8) from the nibble weights
-__device__ static void zb_huf_fill(u16* cells, const u8* ws, u32 log, u32 nsym, const u32* rank, u32 shift, u32 base)
+// fill the decode cells (u16: symbol | nbBits << 8) from the nibble weights.  Every weight's cells start where the runs of
+// the lighter weights end (a prefix over rank); a 16-bit cursor per weight, packed in registers, advances by one run per symbol.
+__device__ static void zb_huf_fill(u16* cells, const u8* ws, u32 log, u32 nsym, ZbRank const& rank, u32 shift, u32 base)
 {
-    u32 start[13]; { u32 p = 0; for (u32 wt = 1; wt <= 12; wt++) { start[wt] = p; p += wt <= log ? (rank[wt] << (wt - 1)) : 0; } }
+    ZbPacked<6, 16> next; next.clear();
+    {
+        u32 p = 0;
+        #pragma unroll
+        for (u32 wt = 1; wt <= 12; wt++) { next.add(wt - 1, p); p += wt <= log ? (rank[wt] << (wt - 1)) : 0; }
+    }
     for (u32 i = 0; i < nsym; i++) {
         u32 const wt = (ws[i >> 1] >> ((i & 1) * 4)) & 15; if (!wt) continue;
-        u32 len = 1u << (wt - 1), p = start[wt]; start[wt] = p + len;
+        u32 len = 1u << (wt - 1), p = next.get(wt - 1); next.add(wt - 1, len);
         if (wt > shift) { len >>= shift; p = base + (p >> shift); }       // coarse part: one cell per 2^shift indices
         u32 const cell = i | ((log + 1 - wt) << 8);
         if (len >= 4) { u64 const v = cell * 0x0001000100010001ull; u64* q = (u64*)(cells + p); for (u32 k = 0; k < len / 4; k++) q[k] = v; }
@@ -171,6 +202,27 @@ __device__ static void zb_huf_fill(u16* cells, const u8* ws, u32 log, u32 nsym, 
         else cells[p] = (u16)cell;
     }
 }
+
+#ifdef ZB_SIMT_EMULATION
+// The CPU build's tests call the Huffman helpers with the weights' counts as u32 rank[0..12] (rank[0]: weight 0); the
+// kernels pass ZbRank.  These adapters exist in that build only.
+__device__ __forceinline__ ZbRank zb_rank_pack(const u32* rank) { ZbRank r; r.clear(); for (u32 wt = 1; wt <= 12; wt++) r.add(wt - 1, rank[wt]); return r; }
+__device__ static u32 zb_huf_weights(u8* ws, const u8* s, u32 n, u32& out_log, u32& out_nsym, u32* rank, ZB_RING_ARG(ring))
+{
+    ZbRank r; u32 const used = zb_huf_weights(ws, s, n, out_log, out_nsym, r, ring);
+    rank[0] = used ? out_nsym : 0;
+    for (u32 w = 1; w <= 12; w++) { rank[w] = used ? r[w] : 0; rank[0] -= rank[w]; }
+    return used;
+}
+__device__ __forceinline__ void zb_huf_shape(u32 log, const u32* rank, u32& shift, u32& T, u32& base, u32& bytes)
+{
+    zb_huf_shape(log, zb_rank_pack(rank), shift, T, base, bytes);
+}
+__device__ static void zb_huf_fill(u16* cells, const u8* ws, u32 log, u32 nsym, const u32* rank, u32 shift, u32 base)
+{
+    zb_huf_fill(cells, ws, log, nsym, zb_rank_pack(rank), shift, base);
+}
+#endif
 
 // one Huffman stream -> n_out bytes at out (global scratch), 4 symbols per 32-bit store where aligned
 __device__ static bool zb_huf_stream2(u8* out, u32 n_out, const u8* s, u32 n, ZbHufTab const t, u8* ring)
@@ -298,6 +350,16 @@ __device__ __forceinline__ u32 zb_ent_head(u8* smem, ZbDictDev const& dict)
     return ((ZB_ENT_SMEM(W) - head) / W) & ~15u;
 }
 
+// per-phase cycle counters (lane 0 of every warp) exist only in tuning builds (-DZB_PHASE_TIMERS)
+#ifdef ZB_PHASE_TIMERS
+__device__ unsigned long long g_zb_ent_phase[8];
+#define ZB_EMARK(k) do { if (lane == 0) { long long const t_ = clock64(); atomicAdd(&g_zb_ent_phase[k], (unsigned long long)(t_ - t_ph)); t_ph = t_; } } while (0)
+#elif defined(ZB_DEBUG_BLOCKS)
+#define ZB_EMARK(k) do { if (err && !(t_ph & 1)) { printf("[emark %d] lane %u err %u\n", k, lane, err); t_ph |= 1; } } while (0)
+#else
+#define ZB_EMARK(k) do { (void)t_ph; } while (0)
+#endif
+
 // -- D of one block in one lane: place the three FSE tables (built at q in the lane's pool claim, or the predefined or the
 // dictionary's ones in the head), then run the 3-state sequence stream (restates ZSTD_decodeSequence, zstd/zstd.c:46862-46986)
 // into sq[0, nseq).  Returns the error code; lit_used / produced / rep0..2 carry the block's totals and repcode history out.
@@ -312,7 +374,7 @@ __device__ __forceinline__ u32 zb_seq_block(const u8* smem, u8* q, u8* ws, ZbDic
                                             ZbTabSrc const& dLL, ZbTabSrc const& dOF, ZbTabSrc const& dML,
                                             u32 msLL, u32 msOF, u32 msML, u32 logLL, u32 logOF, u32 logML,
                                             const u8* ip, const u8* bend, u32 nseq, ZbSeq* sq, u32 n_lit, u64 room, u64 hist,
-                                            u32& rep0, u32& rep1, u32& rep2, u32& lit_used, u32& produced)
+                                            u32& rep0, u32& rep1, u32& rep2, u32& lit_used, u32& produced, long long& t_ph)
 {
     const u32* const lutLL = (const u32*)smem; const u32* const lutML = lutLL + 36;
     short* const normLL = (short*)ws; short* const normOF = normLL + 36; short* const normML = normOF + 32;
@@ -327,6 +389,9 @@ __device__ __forceinline__ u32 zb_seq_block(const u8* smem, u8* q, u8* ws, ZbDic
     setup(dLL, normLL, msLL, logLL, K_LL, dct_ll, dict.ll_log, ZB_ENT_DEF_LL, 6, tLL);
     setup(dOF, normOF, msOF, logOF, K_OF, dct_of, dict.of_log, ZB_ENT_DEF_OF, 5, tOF);
     setup(dML, normML, msML, logML, K_ML, dct_ml, dict.ml_log, ZB_ENT_DEF_ML, 6, tML);
+#ifdef ZB_PHASE_TIMERS
+    { u32 const lane = threadIdx.x & 31; ZB_EMARK(7); }              // the table builds of phase D
+#endif
 
     ZbBitR<8> b;                        // ring: the lane workspace (the normalized counts are consumed)
     if (!b.init(ip, (u32)(bend - ip), ws)) return ZB_E_CORRUPTION;
@@ -391,16 +456,6 @@ __device__ __forceinline__ u32 zb_seq_block(const u8* smem, u8* q, u8* ws, ZbDic
     return err;
 }
 
-// per-phase cycle counters (lane 0 of every warp) exist only in tuning builds (-DZB_PHASE_TIMERS)
-#ifdef ZB_PHASE_TIMERS
-__device__ unsigned long long g_zb_ent_phase[8];
-#define ZB_EMARK(k) do { if (lane == 0) { long long const t_ = clock64(); atomicAdd(&g_zb_ent_phase[k], (unsigned long long)(t_ - t_ph)); t_ph = t_; } } while (0)
-#elif defined(ZB_DEBUG_BLOCKS)
-#define ZB_EMARK(k) do { if (err && !(t_ph & 1)) { printf("[emark %d] lane %u err %u\n", k, lane, err); t_ph |= 1; } } while (0)
-#else
-#define ZB_EMARK(k) do { (void)t_ph; } while (0)
-#endif
-
 template <int ZB_ENT_WARPS>
 __global__ void __launch_bounds__(ZB_ENT_WARPS * 32)
 zb_entropy_decode(const u8* __restrict__ src, const ZbSegment* __restrict__ segs, u32 n_frames,
@@ -413,9 +468,9 @@ zb_entropy_decode(const u8* __restrict__ src, const ZbSegment* __restrict__ segs
     u32 const lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     u32 const pool_bytes = zb_ent_head<ZB_ENT_WARPS>(zb_smem, dict);
     u8* const pool = zb_smem + ZB_ENT_SMEM(ZB_ENT_WARPS) - (ZB_ENT_WARPS - warp) * pool_bytes;      // pools: behind the head
-    u8* const ws = pool + lane * ZB_ENT_WS_BYTES;                       // lane workspace
-    u8* const tabs = pool + 32 * ZB_ENT_WS_BYTES;                       // claimable table space
-    u32 const TAB_BYTES = pool_bytes - 32 * ZB_ENT_WS_BYTES;
+    u8* const ws = pool + lane * ZB_ENT_WS_STRIDE;                       // lane workspace
+    u8* const tabs = pool + 32 * ZB_ENT_WS_STRIDE;                       // claimable table space
+    u32 const TAB_BYTES = pool_bytes - 32 * ZB_ENT_WS_STRIDE;
 
     for (;;) {
         u32 base = 0;
@@ -486,7 +541,7 @@ zb_entropy_decode(const u8* __restrict__ src, const ZbSegment* __restrict__ segs
             }
             ZB_EMARK(1);
             // -- B: literals
-            bool wantH = false; u32 hlog = 0, hns = 0; u32 rank[13]; const u8* hp = nullptr; u32 hleft = 0;
+            bool wantH = false; u32 hlog = 0, hns = 0; ZbRank rank; const u8* hp = nullptr; u32 hleft = 0;
             if (comp) {
                 do {
                     if (L.type == 0) {
@@ -502,7 +557,7 @@ zb_entropy_decode(const u8* __restrict__ src, const ZbSegment* __restrict__ segs
                         hp = bs + L.hdr; hleft = L.csize;
                         if (L.type == 2) { dHuf.kind = ZB_SRC_NCOUNT; dHuf.p = hp; dHuf.n = hleft; }
                         if (dHuf.kind == ZB_SRC_NCOUNT) {
-                            u32 const used = zb_huf_weights(ws, dHuf.p, dHuf.n, hlog, hns, rank, tabs + lane * 64);   // no table lives in the pool during B
+                            u32 const used = zb_huf_weights(ws, dHuf.p, dHuf.n, hlog, hns, rank, tabs + lane * 80);   // no table lives in the pool during B
                             if (used == 0 || (L.type == 2 && used >= hleft)) { err = ZB_E_CORRUPTION; break; }
                             if (L.type == 2) { hp += used; hleft -= used; dHuf.n = used; }
                             wantH = true;
@@ -527,6 +582,7 @@ zb_entropy_decode(const u8* __restrict__ src, const ZbSegment* __restrict__ segs
                     if (pending && incl <= TAB_BYTES) {
                         u16* cells = (u16*)(tabs + incl - ((need + 15) & ~15u));
                         zb_huf_fill(cells, ws, hlog, hns, rank, hshift, hbase);
+                        ZB_EMARK(6);                                   // the Huffman table of phase B; its streams follow
                         ZbHufTab t; t.cells = cells; t.log = hlog; t.shift = hshift; t.T = hT; t.base = hbase;
                         if (!zb_huf_block(lits + lit_i, L.regen, hp, hleft, L.single, t, ws)) { err = ZB_E_CORRUPTION; done = true; comp = false; }
                         pending = false;
@@ -569,12 +625,12 @@ zb_entropy_decode(const u8* __restrict__ src, const ZbSegment* __restrict__ segs
             {
                 bool pending = comp && nseq > 0;
                 while (__any_sync(0xFFFFFFFFu, pending)) {
-                    u32 const need = pending ? ((needS + 15) & ~15u) : 0;
+                    u32 const need = pending ? ZB_ENT_SKEW(needS) : 0;
                     u32 const incl = zb_warp_incl_scan(need, lane);
                     if (pending && incl <= TAB_BYTES) {
                         err = zb_seq_block<false>(zb_smem, tabs + incl - need, ws, dict, dLL, dOF, dML, msLL, msOF, msML, logLL, logOF, logML,
                                                    ip, bend, nseq, seqs + seq_i, L.regen, cap - out_pos, out_pos + hist_extra,
-                                                   rep0, rep1, rep2, lit_used, produced);
+                                                   rep0, rep1, rep2, lit_used, produced, t_ph);
                         if (err) { done = true; comp = false; }
                         pending = false;
                     }
@@ -632,6 +688,7 @@ zb_entropy_blocks(const u8* __restrict__ src, const ZbBlkDesc* __restrict__ bdes
     u32 const lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     u32 const pool_bytes = zb_ent_head<ZB_ENT_WARPS>(zb_smem, dict);
     u8* const pool = zb_smem + ZB_ENT_SMEM(ZB_ENT_WARPS) - (ZB_ENT_WARPS - warp) * pool_bytes;      // pools: behind the head
+    // a few lanes per warp (ZB_BLOCKS_TAKE): no lock-step bank conflicts to spread, so the workspaces are not skewed
     u8* const ws = pool + lane * ZB_ENT_WS_BYTES;                       // lane workspace
     u8* const tabs = pool + 32 * ZB_ENT_WS_BYTES;                       // claimable table space
     u32 const TAB_BYTES = pool_bytes - 32 * ZB_ENT_WS_BYTES;
@@ -705,7 +762,7 @@ zb_entropy_blocks(const u8* __restrict__ src, const ZbBlkDesc* __restrict__ bdes
             }
             ZB_EMARK(1);
             // -- B: literals
-            bool wantH = false; u32 hlog = 0, hns = 0; u32 rank[13]; const u8* hp = nullptr; u32 hleft = 0;
+            bool wantH = false; u32 hlog = 0, hns = 0; ZbRank rank; const u8* hp = nullptr; u32 hleft = 0;
             if (comp) {
                 do {
                     if (L.type == 0) {
@@ -746,6 +803,7 @@ zb_entropy_blocks(const u8* __restrict__ src, const ZbBlkDesc* __restrict__ bdes
                     if (pending && incl <= TAB_BYTES) {
                         u16* cells = (u16*)(tabs + incl - ((need + 15) & ~15u));
                         zb_huf_fill(cells, ws, hlog, hns, rank, hshift, hbase);
+                        ZB_EMARK(6);                                   // the Huffman table of phase B; its streams follow
                         ZbHufTab t; t.cells = cells; t.log = hlog; t.shift = hshift; t.T = hT; t.base = hbase;
                         if (!zb_huf_block(lits + lit_i, L.regen, hp, hleft, L.single, t, ws)) { err = ZB_E_CORRUPTION; done = true; comp = false; }
                         pending = false;
@@ -793,7 +851,7 @@ zb_entropy_blocks(const u8* __restrict__ src, const ZbBlkDesc* __restrict__ bdes
                     if (pending && incl <= TAB_BYTES) {
                         err = zb_seq_block<true>(zb_smem, tabs + incl - need, ws, dict, dLL, dOF, dML, msLL, msOF, msML, logLL, logOF, logML,
                                                    ip, bend, nseq, seqs + seq_i, L.regen, cap - out_pos, out_pos + hist_extra,
-                                                   rep0, rep1, rep2, lit_used, produced);
+                                                   rep0, rep1, rep2, lit_used, produced, t_ph);
                         if (err) { done = true; comp = false; }
                         pending = false;
                     }

@@ -33,9 +33,13 @@ if os.environ.get("PHASES"):
     buf = (C.c_uint64 * 8)(); L.zb_entropy_phase_read(buf, 1)
     xbuf = (C.c_uint64 * 4)(); L.zb_execute_phase_read(xbuf, 1)
     L.zb200_result_free(step()); L.zb_entropy_phase_read(buf, 1); L.zb_execute_phase_read(xbuf, 1)
-    names = ['other/loop', 'A block header', 'B literals hdr+weights', 'huffman table+streams', 'C seq header+ncount', 'D tables+sequences']
-    tot = float(sum(buf[i] for i in range(6))) or 1.0
-    print('entropy phases (share of summed warp cycles):', {nm: "%.1f%%" % (100.0 * buf[i] / tot) for i, nm in enumerate(names)}, "sum Mcycles %.0f" % (tot / 1e6))
+    # slot 6 (Huffman claim + fill) and slot 7 (the three FSE builds) split phases B and D; a lane-0 mark, so when lane 0 has no
+    # Huffman table or no sequences in a round, that round's table time stays with the streams or the sequence loop
+    names = ['other/loop', 'A block header', 'B literals hdr+weights', 'huffman streams', 'C seq header+ncount', 'D sequence loop',
+             'huffman table claim+fill', 'D FSE table builds']
+    tot = float(sum(buf[i] for i in range(8))) or 1.0
+    print('entropy phases (share of summed warp cycles):', {nm: "%.1f%% (%.0f Mcycles)" % (100.0 * buf[i] / tot, buf[i] / 1e6) for i, nm in enumerate(names)},
+          "sum Mcycles %.0f" % (tot / 1e6))
     xnames = ['frame start + literal staging', 'literal copies', 'frontier passes', 'write-out']
     print('zb_execute_tile phases (summed warp cycles):', {nm: "%.1f Mcycles" % (xbuf[i] / 1e6) for i, nm in enumerate(xnames)},
           "sum Mcycles %.0f" % (sum(xbuf[i] for i in range(4)) / 1e6))

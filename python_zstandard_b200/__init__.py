@@ -60,9 +60,11 @@ def frame_header_size(data):
     b = bytes(memoryview(data))
     info = _native.FrameInfo()
     _native.lib().zb200_frame_info(b, len(b), C.byref(info))
-    if info.status:
+    # ZSTD_frameHeaderSize (zstd/zstd.c:43637) looks at no magic number: anything shorter than 5 bytes is srcSize_wrong
+    status = 72 if len(b) < 5 else info.status
+    if status:
         raise ZstdError("could not determine frame header size: %s"
-                        % _native.lib().zb200_error_string(info.status).decode())
+                        % _native.lib().zb200_error_string(status).decode())
     return info.header_size
 
 

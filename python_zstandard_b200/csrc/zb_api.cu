@@ -56,31 +56,30 @@ void zb_launch_finish(const ZbFramePlace* place, const u64* out_sizes, const u32
 void zb_launch_chain_shift(ZbFramePlace* place, u32 n, u64 carry, cudaStream_t st);
 void zb_launch_digest_dict(const u8* dict, u32 n, ZbDictDigest* out, cudaStream_t st);
 size_t zb_encode_scratch_bytes();
-void zb_launch_compress_blocks(const u8* src, const void* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes,
-                               void* outs, u32* work_counter, const u8* dict_tail, u32 dict_D, const u16* dict_table, const void* dict_digest, const void* dict_cct,
+void zb_launch_compress_blocks(const u8* src, const ZeBlockJob* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes,
+                               ZeBlockOut* outs, u32* work_counter, const u8* dict_tail, u32 dict_D, const u16* dict_table, const void* dict_digest, const void* dict_cct,
                                const unsigned long long* upload_progress, unsigned long long upload_total, u32* upload_status, int dual, int small_blocks, cudaStream_t st,
                                u32* stats = nullptr);
 u32 zb_encode_small_max();
 void zb_launch_dict_table(const u8* tail, u32 D, u16* table, cudaStream_t st);
 size_t zb_encode_pscratch_bytes();
-size_t zb_chain_seg_bytes();
-void zb_launch_chain_index(const u8* src, const void* segs, const u64* pos_off, u32 n_segs, u64 total_pos, u32 sms, cudaStream_t st);
-void zb_launch_compress_chain_blocks(const u8* src, const void* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes,
-                                     void* outs, u32* work_counter, const void* segs, cudaStream_t st);
+void zb_launch_chain_index(const u8* src, const ZeChainSeg* segs, const u64* pos_off, u32 n_segs, u64 total_pos, u32 sms, cudaStream_t st);
+void zb_launch_compress_chain_blocks(const u8* src, const ZeBlockJob* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes,
+                                     ZeBlockOut* outs, u32* work_counter, const ZeChainSeg* segs, cudaStream_t st);
 u32 zb_encode_ctable_bytes();
 void zb_launch_dict_ctables(const void* digest, void* out3, cudaStream_t st);
-void zb_launch_frame_layout(const ZbSegment* segs, const void* seginfo, const void* outs, u32 n_segs, u32 checksum, u32 content_size,
+void zb_launch_frame_layout(const ZbSegment* segs, const ZeSegInfo* seginfo, const ZeBlockOut* outs, u32 n_segs, u32 checksum, u32 content_size,
                             u32 dict_id, u32 window_log, u64* sizes, ZbSegment* out_segs, u64* total, cudaStream_t st);
-void zb_launch_write_frames(const u8* src, const ZbSegment* segs, const void* seginfo, const void* outs, const u8* slots, u64 slot_bytes,
+void zb_launch_write_frames(const u8* src, const ZbSegment* segs, const ZeSegInfo* seginfo, const ZeBlockOut* outs, const u8* slots, u64 slot_bytes,
                             u32 n_segs, u32 checksum, u32 content_size, u32 dict_id, u32 window_log, const ZbSegment* out_segs, u8* dst, cudaStream_t st);
 u32 zb_encode_smem_bytes();
 u32 zb_encode3_record_max();
 u32 zb_encode3_records_per_cta();
-void zb_launch_compress_recs(const u8* src, const void* jobs, u32 n_jobs, u32 n_ctas, u8* slots, u64 slot_bytes, void* outs, u32* work_counter,
+void zb_launch_compress_recs(const u8* src, const ZeBlockJob* jobs, u32 n_jobs, u32 n_ctas, u8* slots, u64 slot_bytes, ZeBlockOut* outs, u32* work_counter,
                              const u8* dict_tail, u32 dict_D, const u16* dict_table, const void* dict_digest, const void* dict_cct,
                              const unsigned long long* upload_progress, unsigned long long upload_total, u32* upload_status, cudaStream_t st);
 size_t zb_encode2_scratch_bytes();
-void zb_launch_compress_smem(const u8* src, const void* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes, void* outs, u32* work_counter,
+void zb_launch_compress_smem(const u8* src, const ZeBlockJob* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes, ZeBlockOut* outs, u32* work_counter,
                              const unsigned long long* upload_progress, unsigned long long upload_total, u32* upload_status, cudaStream_t st);
 // dictionary training (zb_train.cuh)
 void zt_launch_hash(const u8* s, u32 n_dmers, u32 f, u32 d, u32* hash, u32 sms, cudaStream_t st);
@@ -696,9 +695,9 @@ int zb200_decompress_chain(zb200_ctx* ctx, const void* const* srcs, const size_t
     for (size_t k = 0; k < n && h == n; k++) {
         const u8* s = (const u8*)srcs[k];
         int code = 0;
-        if (sizes[k] >= 4 && (((u32)s[0] | (u32)s[1] << 8 | (u32)s[2] << 16 | (u32)s[3] << 24) & 0xFFFFFFF0u) == ZB_MAGIC_SKIP) {
+        if (sizes[k] >= 4 && (zb_rd32(s) & 0xFFFFFFF0u) == ZB_MAGIC_SKIP) {
             // a skippable frame first: the reference's stream decoder stops behind it, so the fulltext is empty
-            u64 const len = sizes[k] >= 8 ? ((u32)s[4] | (u32)s[5] << 8 | (u32)s[6] << 16 | (u64)s[7] << 24) : 0;
+            u64 const len = sizes[k] >= 8 ? zb_rd32(s + 4) : 0;
             if (sizes[k] < 8 + len) code = ZB_E_SRCSIZE_WRONG;
             skip[k] = 1;
         } else {
@@ -803,11 +802,6 @@ int zb200_decompress_chain(zb200_ctx* ctx, const void* const* srcs, const size_t
 
 
 // ---------------------------------------------------------------- batch compression
-namespace {
-struct HostJob { u64 src_pos; u32 size, seg, last, first; };
-struct HostSegInfo { u64 first_job; u32 n_jobs, pad; };
-}
-
 // d_stats (dictionary training): u32[377] on the device that the block kernel's STATS instantiation adds its literal and
 // LL / ML / OF code counts to; only zb_compress_blocks has it, so such a call always runs that kernel
 static int compress_common(zb200_ctx* ctx, const void* src_base, const zb200_segment* segs, size_t n,
@@ -849,7 +843,7 @@ static int compress_common(zb200_ctx* ctx, const void* src_base, const zb200_seg
         d_src = ctx->src.as<u8>(); d_segs = ctx->segs.as<ZbSegment>();
     }
     if (zb_trace_on()) tr1 = zb_now_ms();
-    std::vector<HostJob> jobs; std::vector<HostSegInfo> sinfo(n);
+    std::vector<ZeBlockJob> jobs; std::vector<ZeSegInfo> sinfo(n);
     jobs.reserve(n);
     u32 const max_block = zb_cut_blocks(hsegs.data(), n, block_max, jobs, sinfo);
     size_t const nj = jobs.size();
@@ -865,18 +859,18 @@ static int compress_common(zb200_ctx* ctx, const void* src_base, const zb200_seg
     if (recs_kernel) { ctas = (u32)ctx->sm_count; u32 const need = ((u32)nj + zb_encode3_records_per_cta() - 1) / zb_encode3_records_per_cta(); if (ctas > need) ctas = need; }
     if (ctas > nj) ctas = (u32)nj;
     if (ctas == 0) ctas = 1;
-    CK(ctx->jobs.ensure((nj + 1) * sizeof(HostJob)));
-    CK(ctx->seginfo.ensure(n * sizeof(HostSegInfo)));
+    CK(ctx->jobs.ensure((nj + 1) * sizeof(ZeBlockJob)));
+    CK(ctx->seginfo.ensure(n * sizeof(ZeSegInfo)));
     CK(ctx->slots.ensure((nj + 1) * slot_bytes));
-    CK(ctx->bouts.ensure((nj + 1) * 8));
+    CK(ctx->bouts.ensure((nj + 1) * sizeof(ZeBlockOut)));
     if (!recs_kernel) CK(ctx->escratch.ensure((size_t)ctas * (smem_kernel ? zb_encode2_scratch_bytes() : zb_encode_scratch_bytes())));
     CK(ctx->fsizes.ensure(n * sizeof(u64)));
     CK(ctx->out_segs.ensure(n * sizeof(ZbSegment)));
     CK(ctx->small.ensure(256));
     u64* d_total = ctx->small.as<u64>();
     u32* d_counter = (u32*)(d_total + 8);
-    if (nj) CK(cudaMemcpyAsync(ctx->jobs.p, jobs.data(), nj * sizeof(HostJob), cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->seginfo.p, sinfo.data(), n * sizeof(HostSegInfo), cudaMemcpyHostToDevice, ctx->stream));
+    if (nj) CK(cudaMemcpyAsync(ctx->jobs.p, jobs.data(), nj * sizeof(ZeBlockJob), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->seginfo.p, sinfo.data(), n * sizeof(ZeSegInfo), cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemsetAsync(d_counter, 0, 64, ctx->stream));                       // work counter, upload status, upload progress
     u32* const d_upstatus = d_counter + 1;
     unsigned long long* const d_progress = (unsigned long long*)(d_counter + 4);
@@ -901,21 +895,21 @@ static int compress_common(zb200_ctx* ctx, const void* src_base, const zb200_seg
     }
     ctx->last_compress_kernel = recs_kernel ? "zb_compress_recs" : (smem_kernel ? "zb_compress_smem" : "zb_compress_blocks");
     if (recs_kernel) { KSpan s(ctx, ZB200_K_COMPRESS);
-      zb_launch_compress_recs(d_src, ctx->jobs.p, (u32)nj, ctas, ctx->slots.as<u8>(), slot_bytes, ctx->bouts.p, d_counter,
+      zb_launch_compress_recs(d_src, ctx->jobs.as<ZeBlockJob>(), (u32)nj, ctas, ctx->slots.as<u8>(), slot_bytes, ctx->bouts.as<ZeBlockOut>(), d_counter,
                               dict->c_tail, dict->c_D, dict->d_ctable, (const void*)dict->d_digest, dict->d_cct,
                               overlap_upload ? d_progress : nullptr, up_bytes, d_upstatus, ctx->stream); }
     else if (nj && smem_kernel) { KSpan s(ctx, ZB200_K_COMPRESS);
-      zb_launch_compress_smem(d_src, ctx->jobs.p, (u32)nj, ctx->escratch.p, ctas, ctx->slots.as<u8>(), slot_bytes, ctx->bouts.p, d_counter,
+      zb_launch_compress_smem(d_src, ctx->jobs.as<ZeBlockJob>(), (u32)nj, ctx->escratch.p, ctas, ctx->slots.as<u8>(), slot_bytes, ctx->bouts.as<ZeBlockOut>(), d_counter,
                               overlap_upload ? d_progress : nullptr, up_bytes, d_upstatus, ctx->stream); }
     else if (nj) { KSpan s(ctx, ZB200_K_COMPRESS);
-      zb_launch_compress_blocks(d_src, ctx->jobs.p, (u32)nj, ctx->escratch.p, ctas, ctx->slots.as<u8>(), slot_bytes, ctx->bouts.p, d_counter,
+      zb_launch_compress_blocks(d_src, ctx->jobs.as<ZeBlockJob>(), (u32)nj, ctx->escratch.p, ctas, ctx->slots.as<u8>(), slot_bytes, ctx->bouts.as<ZeBlockOut>(), d_counter,
                                 dict ? dict->c_tail : nullptr, dict ? dict->c_D : 0, dict ? dict->d_ctable : nullptr,
                                 (dict && dict->c_D && dict->dev.has_entropy) ? (const void*)dict->d_digest : nullptr, dict ? dict->d_cct : nullptr,
                                 overlap_upload ? d_progress : nullptr, up_bytes, d_upstatus, P.level >= 4 ? 1 : 0, max_block <= zb_encode_small_max() ? 1 : 0, ctx->stream, d_stats); }
     // the layout kernels read the input again (raw blocks): they wait for the whole upload, whatever order the segments came in
     if (overlap_upload) CK(cudaStreamWaitEvent(ctx->stream, ctx->chunk_ev[1], 0));
     { KSpan s(ctx, ZB200_K_LAYOUT);
-      zb_launch_frame_layout(d_segs, ctx->seginfo.p, ctx->bouts.p, (u32)n, P.write_checksum ? 1 : 0, P.write_content_size ? 1 : 0, P.dict_id, P.window_log,
+      zb_launch_frame_layout(d_segs, ctx->seginfo.as<ZeSegInfo>(), ctx->bouts.as<ZeBlockOut>(), (u32)n, P.write_checksum ? 1 : 0, P.write_content_size ? 1 : 0, P.dict_id, P.window_log,
                              ctx->fsizes.as<u64>(), ctx->out_segs.as<ZbSegment>(), d_total, ctx->stream); }
     u64 total = 0; u32 upstatus = 0;
     CK(cudaMemcpyAsync(&total, d_total, sizeof total, cudaMemcpyDeviceToHost, ctx->stream));
@@ -934,7 +928,7 @@ static int compress_common(zb200_ctx* ctx, const void* src_base, const zb200_seg
         d_out = (u8*)p; res->data = p; res->data_on_device = true; res->data_owned_device = true;
     }
     { KSpan s(ctx, ZB200_K_FRAMES);
-      zb_launch_write_frames(d_src, d_segs, ctx->seginfo.p, ctx->bouts.p, ctx->slots.as<u8>(), slot_bytes, (u32)n, P.write_checksum ? 1 : 0,
+      zb_launch_write_frames(d_src, d_segs, ctx->seginfo.as<ZeSegInfo>(), ctx->bouts.as<ZeBlockOut>(), ctx->slots.as<u8>(), slot_bytes, (u32)n, P.write_checksum ? 1 : 0,
                              P.write_content_size ? 1 : 0, P.dict_id, P.window_log, ctx->out_segs.as<ZbSegment>(), d_out, ctx->stream); }
     CK(cudaMemcpyAsync(res->segs.data(), ctx->out_segs.p, n * sizeof(ZbSegment), cudaMemcpyDeviceToHost, ctx->stream));
     if (!(flags & ZB200_DST_DEVICE)) {
@@ -981,16 +975,11 @@ int zb200_compress_batch_ptrs(zb200_ctx* ctx, const void* const* srcs, const siz
 // them is one batch: the chunks back to back on the device (chunk k-1 directly in front of chunk k), an index per chunk
 // (zb_chain_index), every block through the prefix mode of zb_compress_blocks, the frames laid out by the batch kernels with
 // window_log 31 (single segment: the window is the content size, so offsets may reach the whole prefix, RFC 8878 section 3.1.1.1.2).
-namespace {
-struct HostChainSeg { u64 start; const u32* tab; const u32* prev_tab; u32 len, prev_len, log, prev_log; };    // == ZeChainSeg
-}
-
 int zb200_compress_chain(zb200_ctx* ctx, const void* const* srcs, const size_t* sizes, size_t n,
                          const zb200_cparams* params, const zb200_ddict* dict, zb200_result** out)
 {
     *out = nullptr;
     if (!ctx || !srcs || !sizes || n == 0 || n > 0x7FFFFFF0u) return fail(ctx, "zb200_compress_chain: bad arguments", cudaSuccess);
-    if (sizeof(HostChainSeg) != zb_chain_seg_bytes()) return fail(ctx, "zb200_compress_chain: descriptor layout", cudaSuccess);
     for (size_t k = 0; k < n; k++)       // the chain decoder's limit (ZB_FAR_WINDOW); the Python layer checks it first
         if (sizes[k] >= ZB_FAR_WINDOW || (k && sizes[k - 1] + sizes[k] >= ZB_FAR_WINDOW)) return fail(ctx, "zb200_compress_chain: chunk of ZB_FAR_WINDOW or more", cudaSuccess);
     cudaSetDevice(ctx->device);
@@ -1034,20 +1023,20 @@ int zb200_compress_chain(zb200_ctx* ctx, const void* const* srcs, const size_t* 
             if (sizes[k - 1 + i]) memcpy(stage + pos, srcs[k - 1 + i], sizes[k - 1 + i]);
             rsegs[i].offset = pos; rsegs[i].length = sizes[k - 1 + i];
         }
-        std::vector<HostChainSeg> cs(m); std::vector<u64> tab_off(m + 1), pos_off(m + 1);
-        std::vector<HostJob> jobs; std::vector<HostSegInfo> sinfo(m - 1);
+        std::vector<ZeChainSeg> cs(m); std::vector<u64> tab_off(m + 1), pos_off(m + 1);
+        std::vector<ZeBlockJob> jobs; std::vector<ZeSegInfo> sinfo(m - 1);
         zb_chain_plan(rsegs.data(), m, cs.data(), tab_off.data(), pos_off.data(), jobs, sinfo);
         size_t const nj = jobs.size(), nf = m - 1;
         u32 ctas = ctas_max; if (ctas > nj) ctas = (u32)nj; if (ctas == 0) ctas = 1;
         cudaError_t e = ctx->src.ensure(total + 128);
         if (e == cudaSuccess) e = ctx->chain_tab.ensure(tab_off[m] * 4);
-        if (e == cudaSuccess) e = ctx->chain_seg.ensure(m * sizeof(HostChainSeg));
+        if (e == cudaSuccess) e = ctx->chain_seg.ensure(m * sizeof(ZeChainSeg));
         if (e == cudaSuccess) e = ctx->chain_pos.ensure((m + 1) * sizeof(u64));
         if (e == cudaSuccess) e = ctx->segs.ensure(nf * sizeof(ZbSegment));
-        if (e == cudaSuccess) e = ctx->jobs.ensure((nj + 1) * sizeof(HostJob));
-        if (e == cudaSuccess) e = ctx->seginfo.ensure(nf * sizeof(HostSegInfo));
+        if (e == cudaSuccess) e = ctx->jobs.ensure((nj + 1) * sizeof(ZeBlockJob));
+        if (e == cudaSuccess) e = ctx->seginfo.ensure(nf * sizeof(ZeSegInfo));
         if (e == cudaSuccess) e = ctx->slots.ensure((nj + 1) * slot_bytes);
-        if (e == cudaSuccess) e = ctx->bouts.ensure((nj + 1) * 8);
+        if (e == cudaSuccess) e = ctx->bouts.ensure((nj + 1) * sizeof(ZeBlockOut));
         if (e == cudaSuccess) e = ctx->escratch.ensure((size_t)ctas * zb_encode_pscratch_bytes());
         if (e == cudaSuccess) e = ctx->fsizes.ensure(nf * sizeof(u64));
         if (e == cudaSuccess) e = ctx->out_segs.ensure(nf * sizeof(ZbSegment));
@@ -1058,29 +1047,29 @@ int zb200_compress_chain(zb200_ctx* ctx, const void* const* srcs, const size_t* 
         u64* d_total = ctx->small.as<u64>(); u32* d_counter = (u32*)(d_total + 8);
         e = cudaMemcpyAsync(d_src, stage, total + 128, cudaMemcpyHostToDevice, ctx->stream);
         if (e == cudaSuccess) e = cudaMemsetAsync(d_tab, 0xFF, tab_off[m] * 4, ctx->stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->chain_seg.p, cs.data(), m * sizeof(HostChainSeg), cudaMemcpyHostToDevice, ctx->stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->chain_seg.p, cs.data(), m * sizeof(ZeChainSeg), cudaMemcpyHostToDevice, ctx->stream);
         if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->chain_pos.p, pos_off.data(), (m + 1) * sizeof(u64), cudaMemcpyHostToDevice, ctx->stream);
         if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->segs.p, rsegs.data() + 1, nf * sizeof(ZbSegment), cudaMemcpyHostToDevice, ctx->stream);
-        if (e == cudaSuccess && nj) e = cudaMemcpyAsync(ctx->jobs.p, jobs.data(), nj * sizeof(HostJob), cudaMemcpyHostToDevice, ctx->stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->seginfo.p, sinfo.data(), nf * sizeof(HostSegInfo), cudaMemcpyHostToDevice, ctx->stream);
+        if (e == cudaSuccess && nj) e = cudaMemcpyAsync(ctx->jobs.p, jobs.data(), nj * sizeof(ZeBlockJob), cudaMemcpyHostToDevice, ctx->stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->seginfo.p, sinfo.data(), nf * sizeof(ZeSegInfo), cudaMemcpyHostToDevice, ctx->stream);
         if (e == cudaSuccess) e = cudaMemsetAsync(d_counter, 0, 64, ctx->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);          // (the staging block goes back to the pool)
         pinned_put(ctx, stage);
         if (e != cudaSuccess) return fail(ctx, "zb200_compress_chain upload", e);
         { KSpan s(ctx, ZB200_K_CHAIN_INDEX);
-          zb_launch_chain_index(d_src, ctx->chain_seg.p, ctx->chain_pos.as<u64>(), (u32)m, pos_off[m], (u32)ctx->sm_count, ctx->stream); }
+          zb_launch_chain_index(d_src, ctx->chain_seg.as<ZeChainSeg>(), ctx->chain_pos.as<u64>(), (u32)m, pos_off[m], (u32)ctx->sm_count, ctx->stream); }
         if (nj) { KSpan s(ctx, ZB200_K_COMPRESS);
-          zb_launch_compress_chain_blocks(d_src, ctx->jobs.p, (u32)nj, ctx->escratch.p, ctas, ctx->slots.as<u8>(), slot_bytes, ctx->bouts.p, d_counter,
-                                          ctx->chain_seg.p, ctx->stream); }
+          zb_launch_compress_chain_blocks(d_src, ctx->jobs.as<ZeBlockJob>(), (u32)nj, ctx->escratch.p, ctas, ctx->slots.as<u8>(), slot_bytes, ctx->bouts.as<ZeBlockOut>(), d_counter,
+                                          ctx->chain_seg.as<ZeChainSeg>(), ctx->stream); }
         { KSpan s(ctx, ZB200_K_LAYOUT);
-          zb_launch_frame_layout(ctx->segs.as<ZbSegment>(), ctx->seginfo.p, ctx->bouts.p, (u32)nf, P.write_checksum ? 1 : 0, 1, 0, 31,
+          zb_launch_frame_layout(ctx->segs.as<ZbSegment>(), ctx->seginfo.as<ZeSegInfo>(), ctx->bouts.as<ZeBlockOut>(), (u32)nf, P.write_checksum ? 1 : 0, 1, 0, 31,
                                  ctx->fsizes.as<u64>(), ctx->out_segs.as<ZbSegment>(), d_total, ctx->stream); }
         u64 ftotal = 0;
         CK(cudaMemcpyAsync(&ftotal, d_total, sizeof ftotal, cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
         CK(ctx->dst.ensure(ftotal + 64));
         { KSpan s(ctx, ZB200_K_FRAMES);
-          zb_launch_write_frames(d_src, ctx->segs.as<ZbSegment>(), ctx->seginfo.p, ctx->bouts.p, ctx->slots.as<u8>(), slot_bytes, (u32)nf,
+          zb_launch_write_frames(d_src, ctx->segs.as<ZbSegment>(), ctx->seginfo.as<ZeSegInfo>(), ctx->bouts.as<ZeBlockOut>(), ctx->slots.as<u8>(), slot_bytes, (u32)nf,
                                  P.write_checksum ? 1 : 0, 1, 0, 31, ctx->out_segs.as<ZbSegment>(), ctx->dst.as<u8>(), ctx->stream); }
         std::vector<ZbSegment> osegs(nf);
         size_t const base = host.size();
@@ -1141,30 +1130,11 @@ void zb200_result_free(zb200_result* r)
 }
 
 // ---------------------------------------------------------------- frame inspection (host, header only)
-int zb200_frame_info(const void* vsrc, size_t n, zb200_frame_info_t* o)
+int zb200_frame_info(const void* src, size_t n, zb200_frame_info_t* o)
 {
-    // restates ZSTD_getFrameHeader_advanced, zstd/zstd.c:43668-43778 (same rules as zb_parse_header on the device)
-    const u8* s = (const u8*)vsrc;
-    memset(o, 0, sizeof *o); o->content_size = ~0ull;
-    auto rd = [&](size_t p, int k) { u64 v = 0; for (int i = 0; i < k; i++) v |= (u64)s[p + i] << (8 * i); return v; };
-    if (n < 5) { o->status = (n >= 4 && rd(0, 4) != ZB_MAGIC && ((u32)rd(0, 4) & 0xFFFFFFF0u) != ZB_MAGIC_SKIP) ? ZB_E_PREFIX_UNKNOWN : ZB_E_SRCSIZE_WRONG; return 0; }
-    u32 magic = (u32)rd(0, 4);
-    if (magic != ZB_MAGIC) { o->status = ZB_E_PREFIX_UNKNOWN; return 0; }
-    u32 fhd = s[4], single = (fhd >> 5) & 1, did = fhd & 3, fcs = fhd >> 6;
-    u32 need = 5 + (single ? 0 : 1) + (did == 3 ? 4 : did) + (fcs == 0 ? (single ? 1 : 0) : (1u << fcs));
-    if (n < need) { o->status = ZB_E_SRCSIZE_WRONG; return 0; }
-    o->header_size = need;
-    if (fhd & 8) { o->status = ZB_E_FRAMEPARAM_UNSUPPORTED; return 0; }
-    o->has_checksum = (fhd >> 2) & 1;
-    size_t pos = 5;
-    if (!single) { u32 wl = s[pos++], wlog = (wl >> 3) + 10; if (wlog > 31) { o->status = ZB_E_WINDOW_TOO_LARGE; return 0; }
-                   o->window_size = 1ull << wlog; o->window_size += (o->window_size >> 3) * (wl & 7); }
-    if (did) { int k = did == 3 ? 4 : (int)did; o->dict_id = (u32)rd(pos, k); pos += (size_t)k; }
-    if (fcs == 0) { if (single) o->content_size = s[pos]; }
-    else if (fcs == 1) o->content_size = rd(pos, 2) + 256;
-    else if (fcs == 2) o->content_size = rd(pos, 4);
-    else o->content_size = rd(pos, 8);
-    if (single) o->window_size = o->content_size;
+    ZbHdr h; zb_parse_header((const u8*)src, n, h);
+    o->content_size = h.content_size; o->window_size = h.window; o->dict_id = h.dict_id; o->header_size = h.hdr_size;
+    o->has_checksum = h.checksum; o->status = h.status;
     return 0;
 }
 

@@ -5,6 +5,7 @@
 #pragma once
 #include <cstdint>
 #include <cstring>
+#include <vector>
 #include <cuda_runtime.h>
 
 typedef uint8_t  u8;
@@ -59,12 +60,30 @@ struct ZbSegment { u64 offset, length; };       // == BufferSegment, c-ext/pytho
 // 2^window_log bytes, and with them the reach of every match; 0 = the default window
 static inline u32 zb_block_max(u32 window_log) { return window_log && window_log < 17 ? (1u << window_log) : ZB_BLOCK_MAX; }
 
+// ---- the compressor's work records, written by the host (zb_api.cu) and read by the kernels (zb_encode.cu)
+struct ZeBlockJob {        // one <=128 KiB block of one segment
+    u64 src_pos;           // byte position of the block in src
+    u32 size;              // block bytes
+    u32 seg;               // owning segment
+    u32 last;              // last block of its frame
+    u32 first;             // first block of its frame
+};
+struct ZeBlockOut { u32 csize; u32 pad; };     // compressed block bytes (header included) in its slot
+struct ZeSegInfo { u64 first_job; u32 n_jobs; u32 pad; };
+// one chunk of a chain run as the prefix-mode kernel sees it: its bytes, its index, and those of the chunk in front of it
+// (which lies directly in front of it in the run's buffer)
+struct ZeChainSeg {
+    u64 start;                          // byte position of the chunk in src
+    const u32* tab;                     // its index: 2^log u32 slots, the earliest sampled position of every key (two per position)
+    const u32* prev_tab;                // the previous chunk's index (nullptr: none)
+    u32 len, prev_len, log, prev_log;
+};
+
 // The block jobs of a compression call: every <= block_max slice of every segment (ZSTD_compress_frameChunk's block loop,
 // zstd/zstd.c:27545), in segment order, so a job that is not the first of its frame comes right after the one in front of
-// it.  Host code; the launcher and the CPU build of the kernels both cut their jobs here, each with its own structs of the
-// same fields.  Returns the largest block.
-template <class Seg, class JobVec, class InfoVec>
-static inline u32 zb_cut_blocks(const Seg* segs, size_t n, u32 block_max, JobVec& jobs, InfoVec& info)
+// it.  Host code; the launcher and the CPU build of the kernels both cut their jobs here.  Returns the largest block.
+template <class Seg>
+static inline u32 zb_cut_blocks(const Seg* segs, size_t n, u32 block_max, std::vector<ZeBlockJob>& jobs, std::vector<ZeSegInfo>& info)
 {
     u32 max_block = 0;
     for (size_t i = 0; i < n; i++) {
@@ -72,7 +91,7 @@ static inline u32 zb_cut_blocks(const Seg* segs, size_t n, u32 block_max, JobVec
         info[i].first_job = jobs.size(); info[i].n_jobs = 0; info[i].pad = 0;
         while (pos < len) {
             u32 const sz = (u32)(len - pos < block_max ? len - pos : block_max);
-            typename JobVec::value_type j;
+            ZeBlockJob j;
             j.src_pos = segs[i].offset + pos; j.size = sz; j.seg = (u32)i; j.first = pos == 0; j.last = pos + sz == len;
             jobs.push_back(j); info[i].n_jobs++; pos += sz;
             if (sz > max_block) max_block = sz;
@@ -109,8 +128,9 @@ static inline u32 zb_chain_log(u64 len)
 // are the frames' segments.  Fills each chunk's index descriptor except its device pointers (tab, prev_tab), the offsets of
 // the chunks' indexes in the run's slot array (tab_off, m + 1 entries) and of their sampled positions (pos_off, m + 1), and
 // the block jobs of the frames (ZB_BLOCK_MAX blocks, job.seg = the chunk's descriptor) with their layout info (m - 1 entries).
-template <class Seg, class Desc, class JobVec, class InfoVec>
-static inline void zb_chain_plan(const Seg* chunks, size_t m, Desc* cs, u64* tab_off, u64* pos_off, JobVec& jobs, InfoVec& info)
+template <class Seg>
+static inline void zb_chain_plan(const Seg* chunks, size_t m, ZeChainSeg* cs, u64* tab_off, u64* pos_off, std::vector<ZeBlockJob>& jobs,
+                                 std::vector<ZeSegInfo>& info)
 {
     tab_off[0] = pos_off[0] = 0;
     for (size_t i = 0; i < m; i++) {
@@ -248,11 +268,56 @@ struct ZbDictDigest {
     u8 c_huf_nb[256]; u32 c_huf_max;
 };
 
-__device__ __forceinline__ u32 zb_rd16(const u8* p) { return (u32)p[0] | ((u32)p[1] << 8); }
-__device__ __forceinline__ u32 zb_rd24(const u8* p) { return zb_rd16(p) | ((u32)p[2] << 16); }
-__device__ __forceinline__ u32 zb_rd32(const u8* p) { return zb_rd16(p) | (zb_rd16(p + 2) << 16); }
-__device__ __forceinline__ u64 zb_rd64(const u8* p) { return (u64)zb_rd32(p) | ((u64)zb_rd32(p + 4) << 32); }
+__host__ __device__ __forceinline__ u32 zb_rd16(const u8* p) { return (u32)p[0] | ((u32)p[1] << 8); }
+__host__ __device__ __forceinline__ u32 zb_rd24(const u8* p) { return zb_rd16(p) | ((u32)p[2] << 16); }
+__host__ __device__ __forceinline__ u32 zb_rd32(const u8* p) { return zb_rd16(p) | (zb_rd16(p + 2) << 16); }
+__host__ __device__ __forceinline__ u64 zb_rd64(const u8* p) { return (u64)zb_rd32(p) | ((u64)zb_rd32(p + 4) << 32); }
 __device__ __forceinline__ int zb_hibit(u32 v) { return 31 - __clz(v); }
+
+// ---------------------------------------------------------------------------
+// frame header (restates ZSTD_getFrameHeader_advanced, zstd/zstd.c:43668-43778).  The frame scans parse every frame with
+// it on the device, and zb200_frame_info on the host.
+// ---------------------------------------------------------------------------
+struct ZbHdr { u64 content_size; u64 window; u32 dict_id; u32 hdr_size; u32 checksum; u32 status; };
+
+__host__ __device__ static inline void zb_parse_header(const u8* s, u64 n, ZbHdr& h)
+{
+    h.status = ZB_OK; h.content_size = ZB_CONTENT_UNKNOWN; h.window = 0; h.dict_id = 0; h.checksum = 0; h.hdr_size = 0;
+    if (n < 5) {
+        // too short for a header: still report a wrong magic as such (:43680-43697)
+        bool zstd_ok = true, skip_ok = true;
+        const u8 zm[4] = {0x28, 0xB5, 0x2F, 0xFD}, sm[4] = {0x50, 0x2A, 0x4D, 0x18};
+        for (u32 k = 0; k < n && k < 4; k++) {
+            if (s[k] != zm[k]) zstd_ok = false;
+            if (k == 0 ? ((s[0] & 0xF0) != sm[0]) : (s[k] != sm[k])) skip_ok = false;
+        }
+        h.status = (n && !zstd_ok && !skip_ok) ? ZB_E_PREFIX_UNKNOWN : ZB_E_SRCSIZE_WRONG;
+        return;
+    }
+    u32 magic = zb_rd32(s);
+    if (magic != ZB_MAGIC) { h.status = ZB_E_PREFIX_UNKNOWN; return; }
+    u32 fhd = s[4];
+    u32 single = (fhd >> 5) & 1, did = fhd & 3, fcs = fhd >> 6;
+    u32 need = 5 + (single ? 0 : 1) + (did == 3 ? 4 : did) + (fcs == 0 ? (single ? 1 : 0) : (1u << fcs));
+    if (n < need) { h.status = ZB_E_SRCSIZE_WRONG; return; }
+    h.hdr_size = need;
+    if (fhd & 8) { h.status = ZB_E_FRAMEPARAM_UNSUPPORTED; return; }
+    h.checksum = (fhd >> 2) & 1;
+    u32 pos = 5;
+    if (!single) {
+        u32 wl = s[pos++], wlog = (wl >> 3) + 10;
+        if (wlog > 31) { h.status = ZB_E_WINDOW_TOO_LARGE; return; }
+        h.window = 1ull << wlog; h.window += (h.window >> 3) * (wl & 7);
+    }
+    if (did == 1) { h.dict_id = s[pos]; pos += 1; }
+    else if (did == 2) { h.dict_id = zb_rd16(s + pos); pos += 2; }
+    else if (did == 3) { h.dict_id = zb_rd32(s + pos); pos += 4; }
+    if (fcs == 0) { if (single) h.content_size = s[pos]; }
+    else if (fcs == 1) h.content_size = zb_rd16(s + pos) + 256;
+    else if (fcs == 2) h.content_size = zb_rd32(s + pos);
+    else h.content_size = zb_rd64(s + pos);
+    if (single) h.window = h.content_size;
+}
 
 // ---------------------------------------------------------------------------
 // Asynchronous 16-byte global -> shared copies (cp.async.cg: cached in L2 only, never in L1).  The

@@ -49,50 +49,6 @@ __device__ ZbFseCell g_defLL[64];
 __device__ ZbFseCell g_defOF[32];
 __device__ ZbFseCell g_defML[64];
 
-// ---------------------------------------------------------------------------
-// frame header (restates ZSTD_getFrameHeader_advanced, zstd/zstd.c:43668-43778)
-// ---------------------------------------------------------------------------
-struct ZbHdr { u64 content_size; u64 window; u32 dict_id; u32 hdr_size; u32 checksum; u32 status; };
-
-__device__ static void zb_parse_header(const u8* s, u64 n, ZbHdr& h)
-{
-    h.status = ZB_OK; h.content_size = ZB_CONTENT_UNKNOWN; h.window = 0; h.dict_id = 0; h.checksum = 0; h.hdr_size = 0;
-    if (n < 5) {
-        // too short for a header: still report a wrong magic as such (:43680-43697)
-        bool zstd_ok = true, skip_ok = true;
-        const u8 zm[4] = {0x28, 0xB5, 0x2F, 0xFD}, sm[4] = {0x50, 0x2A, 0x4D, 0x18};
-        for (u32 k = 0; k < n && k < 4; k++) {
-            if (s[k] != zm[k]) zstd_ok = false;
-            if (k == 0 ? ((s[0] & 0xF0) != sm[0]) : (s[k] != sm[k])) skip_ok = false;
-        }
-        h.status = (n && !zstd_ok && !skip_ok) ? ZB_E_PREFIX_UNKNOWN : ZB_E_SRCSIZE_WRONG;
-        return;
-    }
-    u32 magic = zb_rd32(s);
-    if (magic != ZB_MAGIC) { h.status = ZB_E_PREFIX_UNKNOWN; return; }
-    u32 fhd = s[4];
-    u32 single = (fhd >> 5) & 1, did = fhd & 3, fcs = fhd >> 6;
-    u32 need = 5 + (single ? 0 : 1) + (did == 3 ? 4 : did) + (fcs == 0 ? (single ? 1 : 0) : (1u << fcs));
-    if (n < need) { h.status = ZB_E_SRCSIZE_WRONG; return; }
-    h.hdr_size = need;
-    if (fhd & 8) { h.status = ZB_E_FRAMEPARAM_UNSUPPORTED; return; }
-    h.checksum = (fhd >> 2) & 1;
-    u32 pos = 5;
-    if (!single) {
-        u32 wl = s[pos++], wlog = (wl >> 3) + 10;
-        if (wlog > 31) { h.status = ZB_E_WINDOW_TOO_LARGE; return; }
-        h.window = 1ull << wlog; h.window += (h.window >> 3) * (wl & 7);
-    }
-    if (did == 1) { h.dict_id = s[pos]; pos += 1; }
-    else if (did == 2) { h.dict_id = zb_rd16(s + pos); pos += 2; }
-    else if (did == 3) { h.dict_id = zb_rd32(s + pos); pos += 4; }
-    if (fcs == 0) { if (single) h.content_size = s[pos]; }
-    else if (fcs == 1) h.content_size = zb_rd16(s + pos) + 256;
-    else if (fcs == 2) h.content_size = zb_rd32(s + pos);
-    else h.content_size = zb_rd64(s + pos);
-    if (single) h.window = h.content_size;
-}
-
 // skip leading skippable frames (ZSTD_decompressMultiFrame, zstd/zstd.c:44318-44330)
 __device__ static bool zb_skip_skippable(const u8*& s, u64& n)
 {

@@ -69,15 +69,6 @@ __constant__ short e_OF_defnorm[29] = {1,1,1,1,1,1,2,2,2,1,1,1,1,1,1,1,1,1,1,1,1
 // ---------------------------------------------------------------------------
 // work description
 // ---------------------------------------------------------------------------
-struct ZeBlockJob {        // one <=128 KiB block of one segment
-    u64 src_pos;           // byte position of the block in src
-    u32 size;              // block bytes
-    u32 seg;               // owning segment
-    u32 last;              // last block of its frame
-    u32 first;             // first block of its frame
-};
-struct ZeBlockOut { u32 csize; u32 pad; };     // compressed block bytes (header included) in its slot
-
 struct ZeParams { u32 checksum; u32 content_size; u32 dict_id; u32 level; u32 window_log = 0; };     // window_log: 0 = default (21)
 
 // dictionary as the block compressor sees it: the last <= 32 KiB of the dictionary content act as history
@@ -109,14 +100,6 @@ struct ZePScratch : ZeScratch {
 };
 static_assert(sizeof(ZePScratch::seqbits) * 8 >= (size_t)ZE_MAXSEQ * ZE_PSEQ_BITS + 26 + 1 + 2 * 32 + 64,
               "the prefix-mode bitstream must hold the worst block: every sequence at its widest, the final states, the zeroed tail");
-// one chunk of a chain run as the prefix-mode kernel sees it: its bytes, its index, and those of the chunk in front of it
-// (which lies directly in front of it in the run's buffer)
-struct ZeChainSeg {
-    u64 start;                          // byte position of the chunk in src
-    const u32* tab;                     // its index: 2^log u32 slots, the earliest sampled position of every key (two per position)
-    const u32* prev_tab;                // the previous chunk's index (nullptr: none)
-    u32 len, prev_len, log, prev_log;
-};
 // The index samples every ZE_CHAIN_STEP-th position (zb_common.cuh).  A slot is keyed on the 8 bytes at a position AND on
 // its 4 KiB bucket: in a revision the bytes of position p mostly sit near p in the previous revision, and a lookup probes the
 // buckets around p.  Keyed on the bytes alone, the earliest occurrence of a common 8-byte string (indentation, a keyword)
@@ -1450,8 +1433,6 @@ zb_chain_index(const u8* __restrict__ src, const ZeChainSeg* __restrict__ segs, 
 // ===========================================================================
 // frame layout
 // ===========================================================================
-struct ZeSegInfo { u64 first_job; u32 n_jobs; u32 pad; };
-
 // frame header bytes for a segment of `size` bytes (restates ZSTD_writeFrameHeader, zstd/zstd.c:27649-27697)
 __device__ __forceinline__ u32 ze_frame_header(u8* o, u64 size, ZeParams P)
 {
@@ -1586,8 +1567,8 @@ size_t zb_encode_scratch_bytes() { return sizeof(ZeScratch); }
 
 void zb_launch_dict_table(const u8* tail, u32 D, u16* table, cudaStream_t st) { ZB_LAUNCH(zb_dict_table, 1, 32, 0, st, tail, D, table); }
 
-void zb_launch_compress_blocks(const u8* src, const void* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes,
-                               void* outs, u32* work_counter, const u8* dict_tail, u32 dict_D, const u16* dict_table, const void* dict_digest, const void* dict_cct,
+void zb_launch_compress_blocks(const u8* src, const ZeBlockJob* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes,
+                               ZeBlockOut* outs, u32* work_counter, const u8* dict_tail, u32 dict_D, const u16* dict_table, const void* dict_digest, const void* dict_cct,
                                const unsigned long long* upload_progress, unsigned long long upload_total, u32* upload_status, int dual, int small_blocks, cudaStream_t st,
                                u32* stats)
 {
@@ -1600,41 +1581,40 @@ void zb_launch_compress_blocks(const u8* src, const void* jobs, u32 n_jobs, void
                         : (small_blocks ? zb_compress_blocks<false, ZE_UNIT_SMALL, true> : zb_compress_blocks<false, ZE_UNIT, true>);
     else k = dual ? (small_blocks ? zb_compress_blocks<true, ZE_UNIT_SMALL, false> : zb_compress_blocks<true, ZE_UNIT, false>)
                   : (small_blocks ? zb_compress_blocks<false, ZE_UNIT_SMALL, false> : zb_compress_blocks<false, ZE_UNIT, false>);
-    ZB_LAUNCH(k, n_ctas, ZE_THREADS, sizeof(ZeShared), st, src, (const ZeBlockJob*)jobs, n_jobs, (ZeScratch*)scratch, slots, slot_bytes,
-              (ZeBlockOut*)outs, work_counter, dict, up, stats);
+    ZB_LAUNCH(k, n_ctas, ZE_THREADS, sizeof(ZeShared), st, src, jobs, n_jobs, (ZeScratch*)scratch, slots, slot_bytes,
+              outs, work_counter, dict, up, stats);
 }
 
 // content-dictionary chains: the chunk indexes of a run, and its block jobs through the prefix mode
 size_t zb_encode_pscratch_bytes() { return sizeof(ZePScratch); }
-size_t zb_chain_seg_bytes() { return sizeof(ZeChainSeg); }
-void zb_launch_chain_index(const u8* src, const void* segs, const u64* pos_off, u32 n_segs, u64 total_pos, u32 sms, cudaStream_t st)
+void zb_launch_chain_index(const u8* src, const ZeChainSeg* segs, const u64* pos_off, u32 n_segs, u64 total_pos, u32 sms, cudaStream_t st)
 {
     if (!total_pos) return;
     u64 const want = (total_pos + 255) / 256; u32 const grid = (u32)(want < (u64)sms * 16 ? want : (u64)sms * 16);
-    ZB_LAUNCH(zb_chain_index, grid, 256, 0, st, src, (const ZeChainSeg*)segs, pos_off, n_segs);
+    ZB_LAUNCH(zb_chain_index, grid, 256, 0, st, src, segs, pos_off, n_segs);
 }
-void zb_launch_compress_chain_blocks(const u8* src, const void* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes,
-                                     void* outs, u32* work_counter, const void* segs, cudaStream_t st)
+void zb_launch_compress_chain_blocks(const u8* src, const ZeBlockJob* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes,
+                                     ZeBlockOut* outs, u32* work_counter, const ZeChainSeg* segs, cudaStream_t st)
 {
     ZeDict dict; memset(&dict, 0, sizeof dict); dict.cct = segs;
     ZeUpload up; up.progress = nullptr; up.total = 0; up.status = nullptr;
-    ZB_LAUNCH((zb_compress_blocks<false, ZE_UNIT, false, true>), n_ctas, ZE_THREADS, sizeof(ZeShared), st, src, (const ZeBlockJob*)jobs, n_jobs,
-              (ZeScratch*)scratch, slots, slot_bytes, (ZeBlockOut*)outs, work_counter, dict, up, nullptr);
+    ZB_LAUNCH((zb_compress_blocks<false, ZE_UNIT, false, true>), n_ctas, ZE_THREADS, sizeof(ZeShared), st, src, jobs, n_jobs,
+              (ZeScratch*)scratch, slots, slot_bytes, outs, work_counter, dict, up, nullptr);
 }
 
-void zb_launch_frame_layout(const ZbSegment* segs, const void* seginfo, const void* outs, u32 n_segs, u32 checksum, u32 content_size,
+void zb_launch_frame_layout(const ZbSegment* segs, const ZeSegInfo* seginfo, const ZeBlockOut* outs, u32 n_segs, u32 checksum, u32 content_size,
                             u32 dict_id, u32 window_log, u64* sizes, ZbSegment* out_segs, u64* total, cudaStream_t st)
 {
     ZeParams P; P.checksum = checksum; P.content_size = content_size; P.dict_id = dict_id; P.level = 3; P.window_log = window_log;
-    ZB_LAUNCH(zb_frame_sizes, (n_segs + 255) / 256, 256, 0, st, segs, (const ZeSegInfo*)seginfo, (const ZeBlockOut*)outs, n_segs, P, sizes);
+    ZB_LAUNCH(zb_frame_sizes, (n_segs + 255) / 256, 256, 0, st, segs, seginfo, outs, n_segs, P, sizes);
     ZB_LAUNCH(zb_scan_sizes, 1, 1024, 0, st, sizes, n_segs, out_segs, total);
 }
 
-void zb_launch_write_frames(const u8* src, const ZbSegment* segs, const void* seginfo, const void* outs, const u8* slots, u64 slot_bytes,
+void zb_launch_write_frames(const u8* src, const ZbSegment* segs, const ZeSegInfo* seginfo, const ZeBlockOut* outs, const u8* slots, u64 slot_bytes,
                             u32 n_segs, u32 checksum, u32 content_size, u32 dict_id, u32 window_log, const ZbSegment* out_segs, u8* dst, cudaStream_t st)
 {
     ZeParams P; P.checksum = checksum; P.content_size = content_size; P.dict_id = dict_id; P.level = 3; P.window_log = window_log;
-    ZB_LAUNCH(zb_write_frames, (n_segs + 7) / 8, 256, 0, st, src, segs, (const ZeSegInfo*)seginfo, (const ZeBlockOut*)outs, slots, slot_bytes, n_segs, P,
+    ZB_LAUNCH(zb_write_frames, (n_segs + 7) / 8, 256, 0, st, src, segs, seginfo, outs, slots, slot_bytes, n_segs, P,
               out_segs, dst);
 }
 
@@ -1643,25 +1623,25 @@ u32 zb_encode_smem_bytes() { return (u32)sizeof(ZeShared); }
 // round-2 kernel: one CTA per SM, block resident in shared memory (no dictionary, blocks compressed independently)
 size_t zb_encode2_scratch_bytes() { return sizeof(Z2Scratch); }
 u32 zb_encode2_smem_bytes() { return (u32)sizeof(Z2Shared); }
-void zb_launch_compress_smem(const u8* src, const void* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes, void* outs, u32* work_counter,
+void zb_launch_compress_smem(const u8* src, const ZeBlockJob* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes, ZeBlockOut* outs, u32* work_counter,
                              const unsigned long long* upload_progress, unsigned long long upload_total, u32* upload_status, cudaStream_t st)
 {
     ZeUpload up; up.progress = upload_progress; up.total = upload_total; up.status = upload_status;
-    ZB_LAUNCH(zb_compress_smem, n_ctas, Z2_NT, sizeof(Z2Shared), st, src, (const ZeBlockJob*)jobs, n_jobs, (Z2Scratch*)scratch, slots, slot_bytes,
-              (ZeBlockOut*)outs, work_counter, up);
+    ZB_LAUNCH(zb_compress_smem, n_ctas, Z2_NT, sizeof(Z2Shared), st, src, jobs, n_jobs, (Z2Scratch*)scratch, slots, slot_bytes,
+              outs, work_counter, up);
 }
 u32 zb_encode_small_max() { return ZE_SMALL_MAX; }
 
 // small records with a full dictionary: a warp per record (zb_encode3.cuh)
 u32 zb_encode3_record_max() { return Z3_RMAX; }
 u32 zb_encode3_records_per_cta() { return Z3_WARPS; }
-void zb_launch_compress_recs(const u8* src, const void* jobs, u32 n_jobs, u32 n_ctas, u8* slots, u64 slot_bytes, void* outs, u32* work_counter,
+void zb_launch_compress_recs(const u8* src, const ZeBlockJob* jobs, u32 n_jobs, u32 n_ctas, u8* slots, u64 slot_bytes, ZeBlockOut* outs, u32* work_counter,
                              const u8* dict_tail, u32 dict_D, const u16* dict_table, const void* dict_digest, const void* dict_cct,
                              const unsigned long long* upload_progress, unsigned long long upload_total, u32* upload_status, cudaStream_t st)
 {
     ZeDict dict; dict.tail = dict_tail; dict.D = dict_D; dict.pad = 0; dict.table = dict_table; dict.ent = (const ZbDictDigest*)dict_digest; dict.cct = dict_cct;
     ZeUpload up; up.progress = upload_progress; up.total = upload_total; up.status = upload_status;
-    ZB_LAUNCH(zb_compress_recs, n_ctas, Z3_NT, sizeof(Z3Shared), st, src, (const ZeBlockJob*)jobs, n_jobs, slots, slot_bytes, (ZeBlockOut*)outs, work_counter,
+    ZB_LAUNCH(zb_compress_recs, n_ctas, Z3_NT, sizeof(Z3Shared), st, src, jobs, n_jobs, slots, slot_bytes, outs, work_counter,
               dict, up);
 }
 u32 zb_encode_ctable_bytes() { return (u32)sizeof(ZeCTable); }

@@ -369,90 +369,124 @@ __device__ unsigned long long g_zb_ent_phase[8];
 // once, after its cell loads, and reads its offset, ML + LL and state bits without refilling in between when they all fit in
 // the window; otherwise it refills before each of the last two reads as well.  Either way every read sees the same bits as
 // with a refill before each read, and left() and its checks are unchanged.
+//
+// Every lane of the warp calls this; the lanes with `go` decode a block, the others only join the warp's stores.  The records
+// are not stored one per lane and sequence: a warp-wide store of 32 lanes' records touches 32 lines.  Each lane stages 8
+// records in ws + 128 (the ring takes ws[0, 128) and nothing else of the workspace is live), and every 8 sequences the warp
+// writes them out together: each 16-byte store instruction carries 4 lanes' runs of 8 consecutive records, 4 to 8 lines.
+// Lanes whose block has ended or failed join those stores with nothing to write.  `ws_stride`: the distance between lanes'
+// workspaces.
 template <bool SYMREP>
-__device__ __forceinline__ u32 zb_seq_block(const u8* smem, u8* q, u8* ws, ZbDictDev const& dict,
+__device__ __forceinline__ u32 zb_seq_block(bool go, const u8* smem, u8* q, u8* ws, u32 ws_stride, ZbDictDev const& dict,
                                             ZbTabSrc const& dLL, ZbTabSrc const& dOF, ZbTabSrc const& dML,
                                             u32 msLL, u32 msOF, u32 msML, u32 logLL, u32 logOF, u32 logML,
                                             const u8* ip, const u8* bend, u32 nseq, ZbSeq* sq, u32 n_lit, u64 room, u64 hist,
                                             u32& rep0, u32& rep1, u32& rep2, u32& lit_used, u32& produced, long long& t_ph)
 {
+    u32 const lane = threadIdx.x & 31;
     const u32* const lutLL = (const u32*)smem; const u32* const lutML = lutLL + 36;
     short* const normLL = (short*)ws; short* const normOF = normLL + 36; short* const normML = normOF + 32;
     u32 const dct_ll = ZB_ENT_HEAD_BYTES, dct_of = dct_ll + (2u << dict.ll_log), dct_ml = dct_of + (2u << dict.of_log);
-    ZbTab tLL, tOF, tML;
+    ZbTab tLL = {0, 0}, tOF = tLL, tML = tLL;
     auto setup = [&](const ZbTabSrc& d, short* norm, u32 ms, u32 lg, int kind, u32 dct, u32 dlog, u32 def, u32 deflog, ZbTab& t) {
         if (d.kind == ZB_SRC_NCOUNT) { zb_build_fse((u16*)q, norm, ms, lg, kind); t.off = (u32)(q - smem); t.log = lg; q += 2u << lg; }
         else if (d.kind == ZB_SRC_RLE) { *(u16*)q = ZB_CELL16(d.sym, 1u); t.off = (u32)(q - smem); t.log = 0; q += 2; }
         else if (d.kind == ZB_SRC_DICT) { t.off = dct; t.log = dlog; }
         else { t.off = def; t.log = deflog; }
     };
-    setup(dLL, normLL, msLL, logLL, K_LL, dct_ll, dict.ll_log, ZB_ENT_DEF_LL, 6, tLL);
-    setup(dOF, normOF, msOF, logOF, K_OF, dct_of, dict.of_log, ZB_ENT_DEF_OF, 5, tOF);
-    setup(dML, normML, msML, logML, K_ML, dct_ml, dict.ml_log, ZB_ENT_DEF_ML, 6, tML);
-#ifdef ZB_PHASE_TIMERS
-    { u32 const lane = threadIdx.x & 31; ZB_EMARK(7); }              // the table builds of phase D
-#endif
-
+    u32 err = ZB_OK;
     ZbBitR<8> b;                        // ring: the lane workspace (the normalized counts are consumed)
-    if (!b.init(ip, (u32)(bend - ip), ws)) return ZB_E_CORRUPTION;
-    u32 sLL = b.read(tLL.log); u32 sOF = b.read(tOF.log); b.refill(); u32 sML = b.read(tML.log);
+    u32 sLL = 0, sOF = 0, sML = 0;
+    if (go) {
+        setup(dLL, normLL, msLL, logLL, K_LL, dct_ll, dict.ll_log, ZB_ENT_DEF_LL, 6, tLL);
+        setup(dOF, normOF, msOF, logOF, K_OF, dct_of, dict.of_log, ZB_ENT_DEF_OF, 5, tOF);
+        setup(dML, normML, msML, logML, K_ML, dct_ml, dict.ml_log, ZB_ENT_DEF_ML, 6, tML);
+#ifdef ZB_PHASE_TIMERS
+        ZB_EMARK(7);                                                  // the table builds of phase D
+#endif
+        if (!b.init(ip, (u32)(bend - ip), ws)) err = ZB_E_CORRUPTION;
+        else { sLL = b.read(tLL.log); sOF = b.read(tOF.log); b.refill(); sML = b.read(tML.log); }
+    }
     const u8* const TL = smem + tLL.off; const u8* const TO = smem + tOF.off; const u8* const TM = smem + tML.off;
     u32 const kL = 31 - tLL.log, kO = 31 - tOF.log, kM = 31 - tML.log;                 // nbBits = clz(x) - k
-    u32 err = ZB_OK;
-    for (u32 i = 0; i < nseq; i++) {
-        u32 const cl = *(const u16*)(TL + 2 * sLL), co = *(const u16*)(TO + 2 * sOF), cm = *(const u16*)(TM + 2 * sML);
-        b.refill();
-        u32 const llc = cl & 63, ofc = co & 63, xl = cl >> 6, xo = co >> 6, xm = cm >> 6;
-        u32 const nl = __clz(xl) - kL, nm = __clz(xm) - kM, no = __clz(xo) - kO;
-        u32 const eL = lutLL[llc], eM = lutML[cm & 63];            // baseline | extra bits << 24: off the state chain
-        u32 const llb = eL >> 24, ab = (eM >> 24) + llb;                                 // ML then LL additional bits (<= 32)
-        u32 const sb = i + 1 < nseq ? nl + nm + no : 0;                                  // the three state updates (<= 26)
-        bool const slow = (int)(ofc + ab + sb) > b.avail;                                 // ofc: the offset's extra bits
-        u32 const ob = b.read(ofc);
-        u32 ll = eL & 0xFFFFFFu, ml = eM & 0xFFFFFFu, off;
-        // (a branch-free select chain over {rep0, rep1, rep2, rep0 - 1, new} was measured 3-5 % slower than this branch)
-        if (ofc > 1) {
-            off = (1u << ofc) - 3 + ob;
-            // SYMREP: bit 31 tags a symbolic history entry, so a concrete offset must stay below 2^31.  The launcher keeps
-            // frames whose window (plus the dictionary) reaches that far off the block path; here such an offset is corrupt.
-            if (SYMREP && (off & 0x80000000u)) { err = ZB_E_CORRUPTION; break; }
-            rep2 = rep1; rep1 = rep0; rep0 = off;
-        } else {
-            u32 const ll0 = (llc == 0);
-            if (ofc == 0) {
-                if (ll0) { off = rep1; rep1 = rep0; rep0 = off; } else off = rep0;
-            } else {
-                u32 const idx = 1 + ll0 + ob;
-                u32 const r0m = SYMREP && (rep0 & 0x80000000u) ? rep0 + 1 : rep0 - 1;   // symbolic: one more off
-                u32 tmp = idx == 1 ? rep1 : (idx == 2 ? rep2 : r0m);
-                // rep0 - 1 == 0 is corrupt (zstd/zstd.c:46905).  SYMREP rejects it here: 0xFFFFFFFF would read as symbolic.
-                if (SYMREP && tmp == 0) { err = ZB_E_CORRUPTION; break; }
-                if (tmp == 0) tmp = 0xFFFFFFFFu;
-                if (idx != 1) rep2 = rep1;
-                rep1 = rep0; rep0 = off = tmp;
+    u8* const stage = ws + 128;
+    bool run = go && !err;
+    u32 i = 0;                                                        // the next sequence
+    for (u32 i0 = 0; __any_sync(0xFFFFFFFFu, run && i0 < nseq); i0 += 8) {
+        bool const ran = run && i0 < nseq;                            // then sq[i0, i) are staged, in slots 0 .. i - i0 - 1
+        if (ran) {
+            while (i < nseq) {
+                u32 const cl = *(const u16*)(TL + 2 * sLL), co = *(const u16*)(TO + 2 * sOF), cm = *(const u16*)(TM + 2 * sML);
+                b.refill();
+                u32 const llc = cl & 63, ofc = co & 63, xl = cl >> 6, xo = co >> 6, xm = cm >> 6;
+                u32 const nl = __clz(xl) - kL, nm = __clz(xm) - kM, no = __clz(xo) - kO;
+                u32 const eL = lutLL[llc], eM = lutML[cm & 63];            // baseline | extra bits << 24: off the state chain
+                u32 const llb = eL >> 24, ab = (eM >> 24) + llb;                                 // ML then LL additional bits (<= 32)
+                u32 const sb = i + 1 < nseq ? nl + nm + no : 0;                                  // the three state updates (<= 26)
+                bool const slow = (int)(ofc + ab + sb) > b.avail;                                 // ofc: the offset's extra bits
+                u32 const ob = b.read(ofc);
+                u32 ll = eL & 0xFFFFFFu, ml = eM & 0xFFFFFFu, off;
+                // (a branch-free select chain over {rep0, rep1, rep2, rep0 - 1, new} was measured 3-5 % slower than this branch)
+                if (ofc > 1) {
+                    off = (1u << ofc) - 3 + ob;
+                    // SYMREP: bit 31 tags a symbolic history entry, so a concrete offset must stay below 2^31.  The launcher keeps
+                    // frames whose window (plus the dictionary) reaches that far off the block path; here such an offset is corrupt.
+                    if (SYMREP && (off & 0x80000000u)) { err = ZB_E_CORRUPTION; break; }
+                    rep2 = rep1; rep1 = rep0; rep0 = off;
+                } else {
+                    u32 const ll0 = (llc == 0);
+                    if (ofc == 0) {
+                        if (ll0) { off = rep1; rep1 = rep0; rep0 = off; } else off = rep0;
+                    } else {
+                        u32 const idx = 1 + ll0 + ob;
+                        u32 const r0m = SYMREP && (rep0 & 0x80000000u) ? rep0 + 1 : rep0 - 1;   // symbolic: one more off
+                        u32 tmp = idx == 1 ? rep1 : (idx == 2 ? rep2 : r0m);
+                        // rep0 - 1 == 0 is corrupt (zstd/zstd.c:46905).  SYMREP rejects it here: 0xFFFFFFFF would read as symbolic.
+                        if (SYMREP && tmp == 0) { err = ZB_E_CORRUPTION; break; }
+                        if (tmp == 0) tmp = 0xFFFFFFFFu;
+                        if (idx != 1) rep2 = rep1;
+                        rep1 = rep0; rep0 = off = tmp;
+                    }
+                }
+                if (slow) b.refill();
+                {
+                    u32 const both = b.read(ab);
+                    ml += both >> llb; ll += both & ((1u << llb) - 1);
+                }
+                if (slow) b.refill();
+                {   // LL, ML, OF in one read
+                    u32 const v = b.read(sb);
+                    sLL = (xl << nl) - (1u << tLL.log) + (v >> (nm + no));
+                    sML = (xm << nm) - (1u << tML.log) + ((v >> no) & ((1u << nm) - 1));
+                    sOF = (xo << no) - (1u << tOF.log) + (v & ((1u << no) - 1));
+                }
+                *(ZbSeq*)(stage + 16 * (i & 7)) = make_uint4(lit_used, produced, ml, off);
+                i++;
+                // the checks of ZSTD_execSequence / ZSTD_execSequenceEnd (zstd/zstd.c:46540-46728)
+                if ((u64)produced + ll + ml > room) { err = ZB_E_DSTSIZE_TOO_SMALL; break; }
+                if (ll > n_lit - lit_used) { err = ZB_E_CORRUPTION; break; }
+                lit_used += ll; produced += ll;
+                if ((u64)off > hist + produced) { err = ZB_E_CORRUPTION; break; }
+                produced += ml;
+                if (!(i & 7)) break;
             }
+            run = !err;
         }
-        if (slow) b.refill();
-        {
-            u32 const both = b.read(ab);
-            ml += both >> llb; ll += both & ((1u << llb) - 1);
+        // the warp's stores: in step j, the 8 lanes of quarter k store record (lane & 7) of lane 4j + k's run.  A run's start
+        // and length travel in one shuffle (ZbSeq is 16-byte aligned, so the pointer's low 4 bits are free for a length <= 8).
+        __syncwarp();
+        u64 const mine = (u64)(uintptr_t)(sq + i0) | (ran ? i - i0 : 0u);
+        u8* const stage0 = stage - lane * ws_stride;
+        u32 const r = lane & 7;
+        #pragma unroll 1
+        for (u32 j = 0; j < 8; j++) {
+            u32 const o = 4 * j + (lane >> 3);
+            u64 const p = __shfl_sync(0xFFFFFFFFu, mine, o);
+            if (r < (u32)(p & 15)) ((ZbSeq*)(uintptr_t)(p & ~15ull))[r] = *(const ZbSeq*)(stage0 + o * ws_stride + 16 * r);
         }
-        if (slow) b.refill();
-        {   // LL, ML, OF in one read
-            u32 const v = b.read(sb);
-            sLL = (xl << nl) - (1u << tLL.log) + (v >> (nm + no));
-            sML = (xm << nm) - (1u << tML.log) + ((v >> no) & ((1u << nm) - 1));
-            sOF = (xo << no) - (1u << tOF.log) + (v & ((1u << no) - 1));
-        }
-        sq[i] = make_uint4(lit_used, produced, ml, off);
-        // the checks of ZSTD_execSequence / ZSTD_execSequenceEnd (zstd/zstd.c:46540-46728)
-        if ((u64)produced + ll + ml > room) { err = ZB_E_DSTSIZE_TOO_SMALL; break; }
-        if (ll > n_lit - lit_used) { err = ZB_E_CORRUPTION; break; }
-        lit_used += ll; produced += ll;
-        if ((u64)off > hist + produced) { err = ZB_E_CORRUPTION; break; }
-        produced += ml;
+        __syncwarp();
     }
-    if (!err && b.left() != 0) err = ZB_E_CORRUPTION;
+    if (go && !err && b.left() != 0) err = ZB_E_CORRUPTION;
     return err;
 }
 
@@ -627,14 +661,15 @@ zb_entropy_decode(const u8* __restrict__ src, const ZbSegment* __restrict__ segs
                 while (__any_sync(0xFFFFFFFFu, pending)) {
                     u32 const need = pending ? ZB_ENT_SKEW(needS) : 0;
                     u32 const incl = zb_warp_incl_scan(need, lane);
-                    if (pending && incl <= TAB_BYTES) {
-                        err = zb_seq_block<false>(zb_smem, tabs + incl - need, ws, dict, dLL, dOF, dML, msLL, msOF, msML, logLL, logOF, logML,
-                                                   ip, bend, nseq, seqs + seq_i, L.regen, cap - out_pos, out_pos + hist_extra,
-                                                   rep0, rep1, rep2, lit_used, produced, t_ph);
+                    bool const go = pending && incl <= TAB_BYTES;
+                    u32 const e = zb_seq_block<false>(go, zb_smem, tabs + incl - need, ws, ZB_ENT_WS_STRIDE, dict, dLL, dOF, dML,
+                                                      msLL, msOF, msML, logLL, logOF, logML, ip, bend, nseq, seqs + seq_i, L.regen,
+                                                      cap - out_pos, out_pos + hist_extra, rep0, rep1, rep2, lit_used, produced, t_ph);
+                    if (go) {
+                        err = e;
                         if (err) { done = true; comp = false; }
                         pending = false;
                     }
-                    __syncwarp();
                 }
             }
             ZB_EMARK(5);
@@ -848,14 +883,15 @@ zb_entropy_blocks(const u8* __restrict__ src, const ZbBlkDesc* __restrict__ bdes
                 while (__any_sync(0xFFFFFFFFu, pending)) {
                     u32 const need = pending ? ((needS + 15) & ~15u) : 0;
                     u32 const incl = zb_warp_incl_scan(need, lane);
-                    if (pending && incl <= TAB_BYTES) {
-                        err = zb_seq_block<true>(zb_smem, tabs + incl - need, ws, dict, dLL, dOF, dML, msLL, msOF, msML, logLL, logOF, logML,
-                                                   ip, bend, nseq, seqs + seq_i, L.regen, cap - out_pos, out_pos + hist_extra,
-                                                   rep0, rep1, rep2, lit_used, produced, t_ph);
+                    bool const go = pending && incl <= TAB_BYTES;
+                    u32 const e = zb_seq_block<true>(go, zb_smem, tabs + incl - need, ws, ZB_ENT_WS_BYTES, dict, dLL, dOF, dML,
+                                                     msLL, msOF, msML, logLL, logOF, logML, ip, bend, nseq, seqs + seq_i, L.regen,
+                                                     cap - out_pos, out_pos + hist_extra, rep0, rep1, rep2, lit_used, produced, t_ph);
+                    if (go) {
+                        err = e;
                         if (err) { done = true; comp = false; }
                         pending = false;
                     }
-                    __syncwarp();
                 }
             }
             ZB_EMARK(5);

@@ -22,6 +22,8 @@
  *   zb200_compress_chain        the per-revision ZSTD_CCtx_refPrefix + ZSTD_compress2 loop that writes such a chain (no entry
  *                               point of the reference; tests/chain_ref.py:compress_chain restates the loop)
  *   zb200_cparams.window_log    ZSTD_c_windowLog of ZstdCompressionParameters   c-ext/compressionparams.c:46
+ *   zb200_cparams.strategy,     ZSTD_c_strategy / _searchLog / _minMatch of ZstdCompressionParameters, greedy to lazy2 only
+ *     .search_log, .min_match   (c-ext/compressionparams.c:198-206)
  *   zb200_host_copy             the write into the result PyBytes   c-ext/decompressor.c:283-352
  *   ZB200_SRC/DST_DEVICE, ZB200_SEGS_HOST, zb200_pointer_device: no counterpart (device-resident callers, SURVEY.md 8(f)-2)
  *
@@ -163,7 +165,13 @@ typedef struct {
     uint32_t dict_id;             /* dictionary id to record, 0 = none (ZSTD_c_dictIDFlag)   */
     uint32_t window_log;          /* 0 = default (21); 10..31: ZSTD_c_windowLog (c-ext/compressionparams.c:46): frames up to 2^W are
                                      single-segment, larger ones declare a 2^W window; blocks are cut to min(2^W, 128 KiB) */
-    uint32_t reserved[3];
+    uint32_t strategy;            /* 0 = the level's own parse; 3 greedy, 4 lazy, 5 lazy2: ZSTD_c_strategy (c-ext/compressionparams.c:206),
+                                     the hash-chain lazy parse of zb_compress_blocks for every block whatever the level, dictionary
+                                     or block size; the other strategies fail the call */
+    uint32_t search_log;          /* with a strategy: 2^min(search_log, 6) chain candidates per position (ZSTD_c_searchLog); 0 = 1,
+                                     level 3's; at most 30 */
+    uint32_t min_match;           /* with a strategy: bytes hashed and shortest match, clamp(min_match, 4, 6) (ZSTD_c_minMatch);
+                                     0 = 5, level 3's; 3..7 */
 } zb200_cparams;
 /* dict: optional dictionary (the same handle decompression uses; compression sees its last <= 32 KiB of
  * content as history before every frame, ZSTD_CCtx_refCDict / loadDictionary_byReference, c-ext/compressor.c:1146-1168) */
@@ -247,8 +255,8 @@ const char* zb200_kernel_name(int k);
 uint64_t zb200_last_scratch_bytes(const zb200_ctx* ctx);
 /* pointer-doubling rounds of the last decompress call that took the pointer-jumping execute stage (0: it did not) */
 int      zb200_last_chase_rounds(const zb200_ctx* ctx);
-/* the block kernel the last compress call ran: "zb_compress_smem", "zb_compress_recs" or "zb_compress_blocks" (they share the
-   profile slot named zb_compress_blocks) */
+/* the block kernel the last compress call ran: "zb_compress_smem", "zb_compress_recs", "zb_compress_blocks" or, with a
+   strategy, "zb_compress_lazy" (the lazy mode of zb_compress_blocks; they all share the profile slot named zb_compress_blocks) */
 const char* zb200_last_compress_kernel(const zb200_ctx* ctx);
 
 #ifdef __cplusplus

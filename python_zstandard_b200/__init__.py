@@ -17,7 +17,10 @@ from .buffers import (BufferSegment, BufferSegments, BufferWithSegments,  # noqa
 from .dictionary import (ZstdCompressionDict, DICT_TYPE_AUTO, DICT_TYPE_RAWCONTENT,  # noqa: F401
                          DICT_TYPE_FULLDICT, train_dictionary)
 from .decompressor import ZstdDecompressor, FORMAT_ZSTD1, FORMAT_ZSTD1_MAGICLESS  # noqa: F401
-from .compressor import ZstdCompressor, ZstdCompressionParameters  # noqa: F401
+from .compressor import (ZstdCompressor, ZstdCompressionParameters,  # noqa: F401
+                         STRATEGY_FAST, STRATEGY_DFAST, STRATEGY_GREEDY, STRATEGY_LAZY, STRATEGY_LAZY2, STRATEGY_BTLAZY2,
+                         STRATEGY_BTOPT, STRATEGY_BTULTRA, STRATEGY_BTULTRA2, SEARCHLOG_MIN, SEARCHLOG_MAX, MINMATCH_MIN,
+                         MINMATCH_MAX, TARGETLENGTH_MIN, TARGETLENGTH_MAX)
 from ._native import set_device, default_device  # noqa: F401
 from .streams import (COMPRESSOBJ_FLUSH_FINISH, COMPRESSOBJ_FLUSH_BLOCK, DECOMPRESSION_RECOMMENDED_INPUT_SIZE,  # noqa: F401
                       DECOMPRESSION_RECOMMENDED_OUTPUT_SIZE, COMPRESSION_RECOMMENDED_INPUT_SIZE,

@@ -20,16 +20,30 @@ from .errors import ZstdError
 
 MAX_COMPRESSION_LEVEL = 22
 
+# the reference's strategy numbers and knob bounds (c-ext/constants.c; zstd.h, 64-bit build)
+STRATEGY_FAST, STRATEGY_DFAST, STRATEGY_GREEDY, STRATEGY_LAZY, STRATEGY_LAZY2 = 1, 2, 3, 4, 5
+STRATEGY_BTLAZY2, STRATEGY_BTOPT, STRATEGY_BTULTRA, STRATEGY_BTULTRA2 = 6, 7, 8, 9
+SEARCHLOG_MIN, SEARCHLOG_MAX = 1, 30
+MINMATCH_MIN, MINMATCH_MAX = 3, 7
+TARGETLENGTH_MIN, TARGETLENGTH_MAX = 0, 131072
+_LAZY_STRATEGIES = (STRATEGY_GREEDY, STRATEGY_LAZY, STRATEGY_LAZY2)
+_OUT_OF_BOUND = "unable to set compression context parameter: Parameter is out of bound"
+
 
 class CParams(C.Structure):
     _fields_ = [("level", C.c_int32), ("write_checksum", C.c_uint32), ("write_content_size", C.c_uint32),
-                ("dict_id", C.c_uint32), ("window_log", C.c_uint32), ("reserved", C.c_uint32 * 3)]
+                ("dict_id", C.c_uint32), ("window_log", C.c_uint32), ("strategy", C.c_uint32), ("search_log", C.c_uint32),
+                ("min_match", C.c_uint32)]
 
 
 class ZstdCompressionParameters:
-    """The subset of c-ext/compressionparams.c that reaches this backend: level, the three frame flags and window_log.
-    The match-finder knobs (hash_log, chain_log, search_log, min_match, target_length, strategy) and the LDM / job knobs
-    configure CPU zstd's strategies, which this backend does not have: anything but their defaults is rejected loudly."""
+    """The subset of c-ext/compressionparams.c that reaches this backend: level, the three frame flags, window_log, and
+    strategy = STRATEGY_GREEDY / STRATEGY_LAZY / STRATEGY_LAZY2 with search_log and min_match, which select the GPU's
+    hash-chain lazy parse (2^min(search_log, 6) chain candidates per position, clamp(min_match, 4, 6)-byte hashes and
+    matches; target_length is accepted and, as in the reference's lazy strategies, has no effect).  Values outside the
+    reference's bounds raise its error.  Any other strategy, search_log / min_match / target_length without one of those
+    three strategies, hash_log, chain_log and the LDM / job knobs configure CPU zstd's other strategies, which this backend
+    does not have: anything but their defaults is rejected loudly."""
 
     _FIELDS = ("format", "compression_level", "window_log", "hash_log", "chain_log", "search_log", "min_match",
                "target_length", "strategy", "write_content_size", "write_checksum", "write_dict_id", "job_size",
@@ -50,13 +64,27 @@ class ZstdCompressionParameters:
         if wl and not (10 <= wl <= 31):
             raise ValueError("window_log out of range")        # ZSTD_c_windowLog bounds, zstd/zstd.c:23003
         self.window_log = wl
+        # ZSTD_CCtxParams_setParameter's bounds (zstd/zstd.c:23763-23783); 0 (and the binding's -1) mean "the level's"
+        given = {k: kw.get(k) for k in ("search_log", "min_match", "target_length", "strategy") if kw.get(k) not in (0, -1, None)}
+        bounds = {"search_log": (SEARCHLOG_MIN, SEARCHLOG_MAX), "min_match": (MINMATCH_MIN, MINMATCH_MAX),
+                  "target_length": (TARGETLENGTH_MIN, TARGETLENGTH_MAX), "strategy": (STRATEGY_FAST, STRATEGY_BTULTRA2)}
+        for k, v in given.items():
+            if not bounds[k][0] <= v <= bounds[k][1]:
+                raise ZstdError(_OUT_OF_BOUND)
+        lazy = given.get("strategy") in _LAZY_STRATEGIES
         for k in ("hash_log", "chain_log", "search_log", "min_match", "target_length", "strategy",
                   "job_size", "overlap_log", "force_max_window", "enable_ldm", "ldm_hash_log", "ldm_min_match",
                   "ldm_bucket_size_log", "ldm_hash_rate_log"):
+            if lazy and k in given:
+                setattr(self, k, given[k])
+                continue
             v = kw.get(k, 0)
             if v not in (0, -1, None):
                 raise ZstdError("compression parameter %s is not supported by the GPU backend" % k)
             setattr(self, k, 0)
+        # What the caller asked for, apart from the attributes: from_level fills the match-finder attributes in as reports
+        # of the reference's choice for the level, and those never select the parse.
+        self._lazy = given["strategy"] if lazy else 0
 
     # The level tables of the reference (zstd/zstd.c:30650-30756): four size classes (any / <= 256 KB / <= 128 KB / <= 16 KB),
     # row 0 = base of the negative levels, rows 1..22 = levels; columns: window_log, chain_log, hash_log, search_log, min_match,
@@ -117,7 +145,9 @@ class ZstdCompressionParameters:
         """ZstdCompressionParameters.from_level (c-ext/compressionparams.c:234-380): the parameters ZSTD_getCParams picks for
         (level, source_size, dict_size), each unless given.  window_log is the one that reaches this backend (frame header,
         block size); the match-finder columns are reported as attributes, like the reference's, and describe CPU strategies
-        this backend replaces by its own parse of that level's class -- asking for DIFFERENT ones is still refused."""
+        this backend replaces by its own parse of that level's class.  An explicit strategy=STRATEGY_GREEDY / _LAZY / _LAZY2
+        keyword selects the GPU's lazy parse, with the search_log and min_match given or else reported for the level; other
+        match-finder keywords are refused as by the constructor."""
         derived = cls._cparams_for(level, source_size, dict_size)
         if kwargs.get("window_log") in (None, 0, -1):
             kwargs["window_log"] = derived["window_log"]
@@ -151,8 +181,12 @@ class ZstdCompressor:
             self._content_size = bool(compression_params.write_content_size)
             self._write_dict_id = bool(compression_params.write_dict_id)
             self._window_log = compression_params.window_log
+            # an explicit greedy / lazy / lazy2 strategy; search_log and min_match 0 take level 3's (1 and 5, zb200.h)
+            lz = compression_params._lazy
+            self._lazy = (lz, compression_params.search_log if lz else 0, compression_params.min_match if lz else 0)
         else:
             self._window_log = 0
+            self._lazy = (0, 0, 0)
             self._level = level
             # defaults: content size on, checksum off, dict id on (c-ext/compressor.c:213-227)
             self._checksum = bool(write_checksum) if write_checksum is not None else False
@@ -163,7 +197,7 @@ class ZstdCompressor:
 
     def _params(self):
         did = self._dict_data.dict_id() if (self._dict_data is not None and self._write_dict_id) else 0
-        return CParams(self._level, int(self._checksum), int(self._content_size), did, self._window_log)
+        return CParams(self._level, int(self._checksum), int(self._content_size), did, self._window_log, *self._lazy)
 
     def _dict(self, ctx):
         return self._dict_data._ddict(ctx) if self._dict_data is not None else None

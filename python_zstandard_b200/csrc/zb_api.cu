@@ -61,6 +61,11 @@ void zb_launch_compress_blocks(const u8* src, const ZeBlockJob* jobs, u32 n_jobs
                                const unsigned long long* upload_progress, unsigned long long upload_total, u32* upload_status, int dual, int small_blocks, cudaStream_t st,
                                u32* stats = nullptr);
 u32 zb_encode_small_max();
+size_t zb_encode_lscratch_bytes();
+void zb_launch_compress_lazy(const u8* src, const ZeBlockJob* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes,
+                             ZeBlockOut* outs, u32* work_counter, const u8* dict_tail, u32 dict_D, const void* dict_digest, const void* dict_cct,
+                             const unsigned long long* upload_progress, unsigned long long upload_total, u32* upload_status,
+                             u32 depth, u32 search_log, u32 min_match, u64 win, cudaStream_t st);
 void zb_launch_dict_table(const u8* tail, u32 D, u16* table, cudaStream_t st);
 size_t zb_encode_pscratch_bytes();
 void zb_launch_chain_index(const u8* src, const ZeChainSeg* segs, const u64* pos_off, u32 n_segs, u64 total_pos, u32 sms, cudaStream_t st);
@@ -813,6 +818,11 @@ static int compress_common(zb200_ctx* ctx, const void* src_base, const zb200_seg
     double const tr0 = zb_trace_on() ? zb_now_ms() : 0; double tr1 = 0, tr2 = 0;
     zb200_cparams P; if (params) P = *params; else { memset(&P, 0, sizeof P); P.level = 3; P.write_content_size = 1; }
     if (P.window_log && (P.window_log < 10 || P.window_log > 31)) return fail(ctx, "zb200_compress_batch: window_log out of range [10, 31]", cudaSuccess);
+    // an explicit strategy: greedy (3), lazy (4) or lazy2 (5) with its search_log and min_match (0: the strategy's own)
+    if (P.strategy && (P.strategy < 3 || P.strategy > 5)) return fail(ctx, "zb200_compress_batch: strategy is not greedy, lazy or lazy2", cudaSuccess);
+    if (P.search_log > 30 || (P.min_match && (P.min_match < 3 || P.min_match > 7)))
+        return fail(ctx, "zb200_compress_batch: search_log or min_match out of range", cudaSuccess);
+    bool const lazy = P.strategy != 0 && !d_stats;
     u32 const block_max = zb_block_max(P.window_log);
     std::vector<zb200_segment> hsegs;
     const u8* d_src; const ZbSegment* d_segs;
@@ -851,9 +861,9 @@ static int compress_common(zb200_ctx* ctx, const void* src_base, const zb200_seg
     // Blocks of 8 KiB and more (no dictionary, level-3 class) take the round-2 kernel: one CTA per SM with the block resident in
     // shared memory.  Small blocks, dictionaries and the level >= 4 mode stay on the CTA-per-block kernel (6 CTAs per SM).
     static int const force_v1 = getenv("ZB200_ENCODER_V1") ? atoi(getenv("ZB200_ENCODER_V1")) : 0;
-    bool const smem_kernel = !dict && P.level < 4 && max_block >= 8192 && !force_v1 && !d_stats;
+    bool const smem_kernel = !lazy && !dict && P.level < 4 && max_block >= 8192 && !force_v1 && !d_stats;
     // Small records with a full dictionary (config 4): a warp per record, 22 records per SM (zb_encode3.cuh).
-    bool const recs_kernel = dict && dict->c_D >= 8 && dict->dev.has_entropy && dict->d_cct && P.level < 4 && nj != 0 &&
+    bool const recs_kernel = !lazy && dict && dict->c_D >= 8 && dict->dev.has_entropy && dict->d_cct && P.level < 4 && nj != 0 &&
                              max_block <= zb_encode3_record_max() && !force_v1 && !d_stats;
     u32 ctas = smem_kernel ? (u32)ctx->sm_count : (u32)ctx->sm_count * (227u * 1024u / zb_encode_smem_bytes());
     if (recs_kernel) { ctas = (u32)ctx->sm_count; u32 const need = ((u32)nj + zb_encode3_records_per_cta() - 1) / zb_encode3_records_per_cta(); if (ctas > need) ctas = need; }
@@ -863,7 +873,8 @@ static int compress_common(zb200_ctx* ctx, const void* src_base, const zb200_seg
     CK(ctx->seginfo.ensure(n * sizeof(ZeSegInfo)));
     CK(ctx->slots.ensure((nj + 1) * slot_bytes));
     CK(ctx->bouts.ensure((nj + 1) * sizeof(ZeBlockOut)));
-    if (!recs_kernel) CK(ctx->escratch.ensure((size_t)ctas * (smem_kernel ? zb_encode2_scratch_bytes() : zb_encode_scratch_bytes())));
+    size_t const scratch_per_cta = recs_kernel ? 0 : (smem_kernel ? zb_encode2_scratch_bytes() : (lazy ? zb_encode_lscratch_bytes() : zb_encode_scratch_bytes()));
+    if (!recs_kernel) CK(ctx->escratch.ensure((size_t)ctas * scratch_per_cta));
     CK(ctx->fsizes.ensure(n * sizeof(u64)));
     CK(ctx->out_segs.ensure(n * sizeof(ZbSegment)));
     CK(ctx->small.ensure(256));
@@ -893,8 +904,14 @@ static int compress_common(zb200_ctx* ctx, const void* src_base, const zb200_seg
         }
         CK(cudaEventRecord(ctx->chunk_ev[1], ctx->copy_stream));
     }
-    ctx->last_compress_kernel = recs_kernel ? "zb_compress_recs" : (smem_kernel ? "zb_compress_smem" : "zb_compress_blocks");
-    if (recs_kernel) { KSpan s(ctx, ZB200_K_COMPRESS);
+    ctx->last_compress_kernel = recs_kernel ? "zb_compress_recs" : (smem_kernel ? "zb_compress_smem" : (lazy ? "zb_compress_lazy" : "zb_compress_blocks"));
+    if (nj && lazy) { KSpan s(ctx, ZB200_K_COMPRESS);
+      zb_launch_compress_lazy(d_src, ctx->jobs.as<ZeBlockJob>(), (u32)nj, ctx->escratch.p, ctas, ctx->slots.as<u8>(), slot_bytes, ctx->bouts.as<ZeBlockOut>(), d_counter,
+                              dict ? dict->c_tail : nullptr, dict ? dict->c_D : 0,
+                              (dict && dict->c_D && dict->dev.has_entropy) ? (const void*)dict->d_digest : nullptr, dict ? dict->d_cct : nullptr,
+                              overlap_upload ? d_progress : nullptr, up_bytes, d_upstatus, P.strategy - 3, P.search_log ? P.search_log : 1u,
+                              P.min_match ? P.min_match : 5u, zb_frame_window(P.window_log, P.write_content_size), ctx->stream); }
+    else if (recs_kernel) { KSpan s(ctx, ZB200_K_COMPRESS);
       zb_launch_compress_recs(d_src, ctx->jobs.as<ZeBlockJob>(), (u32)nj, ctas, ctx->slots.as<u8>(), slot_bytes, ctx->bouts.as<ZeBlockOut>(), d_counter,
                               dict->c_tail, dict->c_D, dict->d_ctable, (const void*)dict->d_digest, dict->d_cct,
                               overlap_upload ? d_progress : nullptr, up_bytes, d_upstatus, ctx->stream); }
@@ -939,7 +956,7 @@ static int compress_common(zb200_ctx* ctx, const void* src_base, const zb200_seg
     }
     CK(cudaStreamSynchronize(ctx->stream));
     if (ctx->prof) fold_spans(ctx);
-    ctx->last_scratch = (recs_kernel ? 0ull : (u64)ctas * (smem_kernel ? zb_encode2_scratch_bytes() : zb_encode_scratch_bytes())) + nj * slot_bytes;
+    ctx->last_scratch = (u64)ctas * scratch_per_cta + nj * slot_bytes;
     if (zb_trace_on()) { double const tr3 = zb_now_ms();
         fprintf(stderr, "[zb200] compress ctx %p n=%zu blocks=%zu: start %.3f upload %.2f kernels %.2f frames+download %.2f ms\n",
                 (void*)ctx, n, nj, tr0, tr1 - tr0, tr2 - tr1, tr3 - tr2); }

@@ -59,6 +59,14 @@ struct ZbSegment { u64 offset, length; };       // == BufferSegment, c-ext/pytho
 // Block_Maximum_Size = min(window, 128 KiB) (ZSTD_getBlockSize, zstd/zstd.c:27478): a window_log below 17 cuts blocks of
 // 2^window_log bytes, and with them the reach of every match; 0 = the default window
 static inline u32 zb_block_max(u32 window_log) { return window_log && window_log < 17 ? (1u << window_log) : ZB_BLOCK_MAX; }
+// The window a frame of more than one block declares (ze_frame_header): 2^W with a content size (W = window_log, 21 when
+// 0; a single-segment frame's window is its content size, which no offset inside the frame exceeds either), else
+// 2^min(W, 17).  The lazy mode keeps the offsets of a frame's later blocks within it.
+static inline u64 zb_frame_window(u32 window_log, u32 content_size)
+{
+    u32 const wl = window_log ? window_log : 21u;
+    return 1ull << (content_size ? wl : (wl < 17 ? wl : 17u));
+}
 
 // ---- the compressor's work records, written by the host (zb_api.cu) and read by the kernels (zb_encode.cu)
 struct ZeBlockJob {        // one <=128 KiB block of one segment

@@ -100,6 +100,14 @@ struct ZePScratch : ZeScratch {
 };
 static_assert(sizeof(ZePScratch::seqbits) * 8 >= (size_t)ZE_MAXSEQ * ZE_PSEQ_BITS + 26 + 1 + 2 * 32 + 64,
               "the prefix-mode bitstream must hold the worst block: every sequence at its widest, the final states, the zeroed tail");
+// Lazy mode (explicit greedy / lazy / lazy2 strategy): a ZePScratch per CTA -- dist32 holds the hash-chain link of every
+// block position, seqml / seqbits as in the prefix mode -- followed by the links of the history positions in front of the
+// block (up to one block), ZE_LSCRATCH bytes per CTA in all.
+#define ZE_LSCRATCH (sizeof(ZePScratch) + (size_t)ZE_BLOCK * 4)
+// what the lazy mode is asked for: depth 0 greedy, 1 lazy, 2 lazy2; chain candidates tried per position; bytes hashed and
+// shortest match (4..6); the largest offset a block that is not its frame's first may use (the window its frame declares)
+struct ZeLazy { u32 depth; u32 attempts; u32 mls; u32 win; };
+#define ZE_LHLOG 13                     // lazy mode: 2^13 u32 chain heads in the 32 KB of the hash-head table
 // The index samples every ZE_CHAIN_STEP-th position (zb_common.cuh).  A slot is keyed on the 8 bytes at a position AND on
 // its 4 KiB bucket: in a revision the bytes of position p mostly sit near p in the previous revision, and a lookup probes the
 // buckets around p.  Keyed on the bytes alone, the earliest occurrence of a common 8-byte string (indentation, a keyword)
@@ -579,16 +587,27 @@ __device__ __forceinline__ u32 ze_rec_off(u32 off, u32 ll, u32& r0, u32& r1, u32
 // is a lookup of every position's 8-byte hash in the two chunk indexes (zb_chain_index) instead of the hash links; the
 // parse runs as in the other modes on 32-bit distances; the compaction merges matches that continue across unit borders
 // and re-derives the repcodes of the whole block; scratch is a ZePScratch array.
-template <bool DUAL, u32 UNIT, bool STATS = false, bool PREFIX = false>
+// LAZY (an explicit greedy / lazy / lazy2 strategy, DUAL false, UNIT 1 KiB; `lz` says which): the reference's hash-chain
+// lazy parse (ZSTD_compressBlock_lazy_generic, zstd/zstd.c:34190).  A block that is not its frame's first has up to one
+// previous block of the frame in front of it as history, as far back as lz.win allows; a first block has the dictionary
+// tail.  Phase A links every position of history and block to the previous one with the same lz.mls-byte hash (32-bit
+// distances); phase C walks those chains, lz.attempts candidates per position, with repcodes first and the reference's
+// lazy gain rule; phases D-F are the prefix mode's (records with raw offsets, merged and coded per block).  Scratch is
+// ZE_LSCRATCH bytes per CTA.
+template <bool DUAL, u32 UNIT, bool STATS = false, bool PREFIX = false, bool LAZY = false>
 __global__ void __launch_bounds__(ZE_THREADS)
 zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jobs, u32 n_jobs,
                    ZeScratch* __restrict__ scratch, u8* __restrict__ slots, u64 slot_bytes,
-                   ZeBlockOut* __restrict__ outs, u32* __restrict__ work_counter, ZeDict dict, ZeUpload up, u32* __restrict__ stats = nullptr)
+                   ZeBlockOut* __restrict__ outs, u32* __restrict__ work_counter, ZeDict dict, ZeUpload up, u32* __restrict__ stats,
+                   ZeLazy lz)
 {
+    constexpr bool WIDE = PREFIX || LAZY;       // records keep raw offsets, 32-bit match lengths and the wide bitstream
     ZB_DYN_SMEM(ze_smem_raw);
     ZeShared& S = *(ZeShared*)ze_smem_raw;
-    ZeScratch& G = PREFIX ? (ZeScratch&)((ZePScratch*)scratch)[blockIdx.x] : scratch[blockIdx.x];
-    ZePScratch& GP = (ZePScratch&)G;            // (PREFIX only)
+    ZeScratch& G = PREFIX ? (ZeScratch&)((ZePScratch*)scratch)[blockIdx.x]
+                          : (LAZY ? *(ZeScratch*)((u8*)scratch + (size_t)blockIdx.x * ZE_LSCRATCH) : scratch[blockIdx.x]);
+    ZePScratch& GP = (ZePScratch&)G;            // (PREFIX and LAZY only)
+    u32* const hlink = (u32*)(&GP + 1);         // (LAZY only) the links of the history positions
     u32 const tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     __shared__ u32 s_job;
 
@@ -629,9 +648,11 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
         ZeChainSeg cs = {}; if constexpr (PREFIX) cs = ((const ZeChainSeg*)dict.cct)[job.seg];
         u32 const bpos = PREFIX ? (u32)(job.src_pos - cs.start) : 0u;             // (PREFIX) block position in its chunk
         // PREFIX: everything in front of the block back to the start of the previous chunk is history
-        u32 const D = PREFIX ? bpos + cs.prev_len : (job.first ? dict.D : (hist ? ZE_HIST : 0u));
-        const u8* const dict_end = (PREFIX || hist) ? in : dict.tail + dict.D;
-        bool const dict_first = PREFIX ? false : (DUAL ? job.first != 0 : true);  // dictionary entropy tables / repcodes belong to first blocks only
+        // LAZY: the previous block of the frame (a full block_max), as far back as the frame's window allows
+        u32 const lhist = LAZY && !job.first ? min(jobs[j - 1].size, lz.win) : 0u;
+        u32 const D = PREFIX ? bpos + cs.prev_len : (job.first ? dict.D : (hist ? ZE_HIST : lhist));
+        const u8* const dict_end = (PREFIX || hist || lhist) ? in : dict.tail + dict.D;
+        bool const dict_first = PREFIX ? false : (DUAL || LAZY ? job.first != 0 : true);  // dictionary entropy tables / repcodes belong to first blocks only
         bool const skip0 = job.first && D == 0;                    // without a dictionary the reference never uses position 0 as a match source
         u32 const n = job.size;
         constexpr u32 unit = UNIT;                                 // bytes each parse lane owns
@@ -663,7 +684,7 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
         ZE_MARK(0);
         // ---------------- A: hash links (warp 0); the other warps clear the histograms meanwhile
         if constexpr (!PREFIX) {
-        if (D && !hist) { const u32* t32 = (const u32*)dict.table; for (u32 i = tid; i < (1u << ZE_HLOG) / 2; i += ZE_THREADS) ((u32*)S.head)[i] = t32[i]; }
+        if (!LAZY && D && !hist) { const u32* t32 = (const u32*)dict.table; for (u32 i = tid; i < (1u << ZE_HLOG) / 2; i += ZE_THREADS) ((u32*)S.head)[i] = t32[i]; }
         else for (u32 i = tid; i < (1u << ZE_HLOG) / 2; i += ZE_THREADS) ((u32*)S.head)[i] = 0xFFFFFFFFu;
         }
         for (u32 i = tid; i < 256; i += ZE_THREADS) S.hist[i] = 0;
@@ -711,7 +732,36 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
             }
             __syncthreads();
         }
-        if (!PREFIX && warp == 0) {
+        if constexpr (LAZY) { if (warp == 0) {
+            // hash chains over history + block (virtual position v = D + block position): 32 positions per step, each links
+            // to the nearest earlier position with the same hash -- a lower lane of the same step (match.any) or the head.
+            // Exact, so the chains do not depend on timing.  The heads are 2^ZE_LHLOG u32 in the hash-head table's storage.
+            u32* const head = (u32*)S.head;
+            u32 const lt = (1u << lane) - 1, total = D + n;
+            u64 const mask = (1ull << (8 * lz.mls)) - 1;
+            for (u32 b = 0; b < total; b += 32) {
+                u32 const v = b + lane;
+                bool const valid = v + lz.mls <= total && !(skip0 && v == 0);
+                u32 h = 0;
+                if (valid) {
+                    int const p = (int)v - (int)D;                           // block position; negative: history
+                    u64 x = 0;
+                    if (p >= 0 ? (u32)p + 12 <= n : p + 12 <= 0) x = ze_ld64(p >= 0 ? in + p : dict_end + p);   // (16 bytes of slack behind a dictionary tail)
+                    else for (u32 k = 0; k < lz.mls; k++) { int const q = p + (int)k; x |= (u64)(q >= 0 ? in[q] : dict_end[q]) << (8 * k); }
+                    h = (u32)(((x & mask) * 0xCF1BBCDCB7A56463ull) >> (64 - ZE_LHLOG));
+                }
+                u32 const m = __match_any_sync(0xFFFFFFFFu, valid ? h : (0x10000u + lane));
+                u32 const lower = m & lt;
+                u32 prev = 0xFFFFFFFFu;
+                if (valid) prev = lower ? b + 31 - __clz(lower) : head[h];
+                ZB_SIMT_STEP();
+                if (valid && (m >> lane) == 1u) head[h] = v;                 // the highest lane of a group owns the slot
+                u32 const lk = prev != 0xFFFFFFFFu ? v - prev : 0u;
+                if (v < D) hlink[v] = lk; else if (v < total) GP.dist32[v - D] = lk;
+                __syncwarp();
+            }
+        } }
+        if (!PREFIX && !LAZY && warp == 0) {
             u32 const lt = (1u << lane) - 1;
             volatile u16* const vhead = S.head;      // one warp, converged every step: table accesses stay in program order
             bool const exact = n < 2048;
@@ -865,6 +915,87 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
         // candidate bytes at ip and ip+1, both repcode candidates, the backward bytes, the next dist
         // entry) and then decides, so a step costs one memory round trip for the whole warp instead of
         // one per divergent path.  Long matches continue in EXTEND iterations, 8 bytes per step.
+        // LAZY: a lane per 1 KiB unit walks its unit serially, as ZSTD_compressBlock_lazy_generic walks a block.
+        if constexpr (LAZY) {
+            u32 const u0 = tid * unit;
+            u32 cnt = 0, tail = 0;
+            if (u0 < n) {
+                u32 const end = min(u0 + unit, n), mls = lz.mls;
+                bool const contiguous = dict_end == in;                     // history directly in front of the block
+                uint2* const rec = G.useq + tid * ZE_UNIT_SEQ;
+                u32 r0 = 0, r1 = 0, r2 = 0;                                  // the unit's own repcodes (phase D codes the block's)
+                if (tid == 0 && dict_first && D && dict.ent) { r0 = dict.ent->rep[0]; r1 = dict.ent->rep[1]; r2 = dict.ent->rep[2]; }
+                // the largest offset a match at p may have: back to the start of the history, and within the window in a block
+                // that follows another of its frame (a first block's history is the dictionary, which the window does not bound)
+                auto max_off = [&](u32 p) { return job.first ? p + D : min(lz.win, p + D); };
+                // bytes in common at p and p - off, at most `limit` (p + limit <= n); the source may start in a separate dictionary
+                // tail and run on into the block
+                auto mcount = [&](u32 p, u32 off, u32 limit) -> u32 {
+                    int const q = (int)p - (int)off;
+                    if (q >= 0 || contiguous) return ze_count(in + p, in + q, limit);
+                    u32 const l1 = min(limit, (u32)(-q));
+                    u32 const m = ze_count(in + p, dict_end + q, l1);
+                    return m == l1 && l1 < limit ? m + ze_count(in + p + m, in, limit - m) : m;
+                };
+                auto link = [&](u32 v) -> u32 { return v < D ? hlink[v] : GP.dist32[v - D]; };
+                // longest match of at least mls bytes at p among lz.attempts chain candidates (0: none); offset in `off`
+                auto search = [&](u32 p, u32& off) -> u32 {
+                    u32 best = 0; off = 0;
+                    if (p + mls > end) return 0;
+                    u32 const v = p + D, lim = max_off(p), room = end - p;
+                    u32 cur = v;
+                    for (u32 a = 0; a < lz.attempts; a++) {
+                        u32 const l = link(cur);
+                        if (!l || v - (cur - l) > lim) break;
+                        cur -= l;
+                        u32 const m = mcount(p, v - cur, room);
+                        if (m > best) { best = m; off = v - cur; if (m == room) break; }
+                    }
+                    return best >= mls ? best : 0;
+                };
+                auto rep_len = [&](u32 p, u32 off) -> u32 {               // a repcode match at p: its length, 0 if under 4 bytes
+                    if (!off || off > max_off(p) || p + 4 > end) return 0;
+                    u32 const m = mcount(p, off, end - p);
+                    return m >= 4 ? m : 0;
+                };
+                u32 ip = u0, anchor = u0;
+                if (ip == 0 && skip0) ip = 1;                                // the reference starts its search at position 1
+                while (ip + mls <= end) {
+                    // repcode at ip + 1, then the chain at ip (zstd/zstd.c:34190-34215)
+                    u32 ml = rep_len(ip + 1, r0), ob = 1, start = ip + 1;
+                    bool searched = false;
+                    { u32 off; u32 const m2 = search(ip, off); if (m2 > ml) { ml = m2; ob = off + 3; start = ip; searched = true; } }
+                    if (ml < 4) { ip += ((ip - anchor) >> 8) + 1; continue; }
+                    // lazy evaluation at the next positions: the gain rule of zstd/zstd.c:34217-34265
+                    u32 p = ip;
+                    for (u32 depth = 1; depth <= lz.depth && p + 1 + mls <= end;) {
+                        p++;
+                        u32 const mr = ob != 1 || start != p ? rep_len(p, r0) : 0;
+                        if (mr && (int)(mr * (depth == 1 ? 3 : 4)) > (int)(ml * (depth == 1 ? 3 : 4)) - (int)ze_hibit(ob) + 1) {
+                            ml = mr; ob = 1; start = p; searched = false;
+                        }
+                        u32 off; u32 const m2 = search(p, off);
+                        if (m2 >= 4 && (int)(m2 * 4) - (int)ze_hibit(off + 3) > (int)(ml * 4) - (int)ze_hibit(ob) + (depth == 1 ? 4 : 7)) {
+                            ml = m2; ob = off + 3; start = p; searched = true; depth = 1; continue;
+                        }
+                        depth++;
+                    }
+                    u32 const off = ob == 1 ? r0 : ob - 3;
+                    if (searched)                                            // catch up: extend backwards (zstd/zstd.c:34280)
+                        while (start > anchor && off < start + D && in[start - 1] == ((int)(start - 1) - (int)off >= 0 ? in[start - 1 - off] : dict_end[(int)(start - 1) - (int)off])) { start--; ml++; }
+                    u32 const ll = start - anchor;
+                    rec[cnt++] = make_uint2(ll | (ml << 16), ze_rec_off<true>(off, ll, r0, r1, r2));
+                    ip = anchor = start + ml;
+                    // immediate repcode: the second most recent offset, no literals
+                    for (u32 mr; ip + mls <= end && (mr = rep_len(ip, r1)) != 0;) {
+                        rec[cnt++] = make_uint2(mr << 16, ze_rec_off<true>(r1, 0, r0, r1, r2));
+                        ip = anchor = ip + mr;
+                    }
+                }
+                tail = end - anchor;
+            }
+            S.ucnt[tid] = (u16)cnt; S.utail[tid] = (u16)tail;
+        } else
         {
             auto dist_at = [&](u32 i) -> u32 { if constexpr (PREFIX) return GP.dist32[i]; else return G.dist[i]; };
             u32 const u0 = tid * unit;
@@ -1053,7 +1184,7 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
         ZE_MARK(2);
         // ---------------- D: compaction of the units' sequences + literal gather
         u32 nseq;
-        if constexpr (PREFIX) {
+        if constexpr (WIDE) {
             // One serial pass: a unit's leading match that continues the previous unit's trailing match (same offset, no
             // literals between) is merged into it -- a revision that is one long match stays one sequence, not one per
             // 1 KiB unit -- and every offset is coded against the block's own repcode history.  Repcodes start as zeros,
@@ -1105,7 +1236,7 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
             for (u32 base = 0; base < nseq; base += ZE_THREADS) {
                 u32 const i = base + tid; bool const v = i < nseq;
                 uint2 const r = v ? G.seq[i] : make_uint2(0, 0);
-                u32 const ll = r.x, ml = PREFIX ? (v ? GP.seqml[i] : 0u) : r.y >> 20, ob = PREFIX ? r.y : r.y & 0xFFFFFu;
+                u32 const ll = r.x, ml = WIDE ? (v ? GP.seqml[i] : 0u) : r.y >> 20, ob = WIDE ? r.y : r.y & 0xFFFFFu;
                 u32 tot_l, tot_s;
                 u32 const lpos = ze_block_scan(ll, S.s_warp, tot_l) + lit_run;
                 u32 const spos = ze_block_scan(ll + ml, S.s_warp, tot_s) + src_run;
@@ -1217,8 +1348,8 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
         }
 
         ZE_MARK(5);
-        // ---------------- E: sequences -> tmp_seq (PREFIX: seqbits)
-        u32* const tseq = PREFIX ? GP.seqbits : G.tmp_seq;
+        // ---------------- E: sequences -> tmp_seq (WIDE: seqbits)
+        u32* const tseq = WIDE ? GP.seqbits : G.tmp_seq;
         u32 seq_payload = 0;
         if (nseq) {
             // three state chains, last sequence to first (warps 0..2, lane 0)
@@ -1279,7 +1410,7 @@ zb_compress_blocks(const u8* __restrict__ src, const ZeBlockJob* __restrict__ jo
             __syncthreads();
             for (u32 i = tid; i < nseq; i += ZE_THREADS) {
                 uint2 const r = G.seq[i];
-                u32 const ll = r.x, ml = (PREFIX ? GP.seqml[i] : r.y >> 20) - 3, ob = PREFIX ? r.y : r.y & 0xFFFFFu;
+                u32 const ll = r.x, ml = (WIDE ? GP.seqml[i] : r.y >> 20) - 3, ob = WIDE ? r.y : r.y & 0xFFFFFu;
                 u32 bp = G.bitpos[i];
                 u32 const so = G.sbits[1][i], sm = G.sbits[2][i], sl = G.sbits[0][i];
                 ze_put_bits(tseq, bp, so & 0xFFF, so >> 12); bp += so >> 12;     // OF, ML, LL state bits
@@ -1582,7 +1713,25 @@ void zb_launch_compress_blocks(const u8* src, const ZeBlockJob* jobs, u32 n_jobs
     else k = dual ? (small_blocks ? zb_compress_blocks<true, ZE_UNIT_SMALL, false> : zb_compress_blocks<true, ZE_UNIT, false>)
                   : (small_blocks ? zb_compress_blocks<false, ZE_UNIT_SMALL, false> : zb_compress_blocks<false, ZE_UNIT, false>);
     ZB_LAUNCH(k, n_ctas, ZE_THREADS, sizeof(ZeShared), st, src, jobs, n_jobs, (ZeScratch*)scratch, slots, slot_bytes,
-              outs, work_counter, dict, up, stats);
+              outs, work_counter, dict, up, stats, ZeLazy{});
+}
+
+// an explicit greedy (depth 0), lazy (1) or lazy2 (2) strategy: the lazy mode of the block kernel, ZE_LSCRATCH bytes of scratch
+// per CTA.  search_log 1.., min_match as given; win: the largest offset of a block behind its frame's first (the frame's window).
+size_t zb_encode_lscratch_bytes() { return ZE_LSCRATCH; }
+void zb_launch_compress_lazy(const u8* src, const ZeBlockJob* jobs, u32 n_jobs, void* scratch, u32 n_ctas, u8* slots, u64 slot_bytes,
+                             ZeBlockOut* outs, u32* work_counter, const u8* dict_tail, u32 dict_D, const void* dict_digest, const void* dict_cct,
+                             const unsigned long long* upload_progress, unsigned long long upload_total, u32* upload_status,
+                             u32 depth, u32 search_log, u32 min_match, u64 win, cudaStream_t st)
+{
+    ZeDict dict; dict.tail = dict_tail; dict.D = dict_D; dict.pad = 0; dict.table = nullptr; dict.ent = (const ZbDictDigest*)dict_digest; dict.cct = dict_digest ? dict_cct : nullptr;
+    ZeUpload up; up.progress = upload_progress; up.total = upload_total; up.status = upload_status;
+    // 2^min(search_log, 6) candidates (the row-based finder's cap, zstd/zstd.c:33870); clamp(min_match, 4, 6) bytes
+    // (ZSTD_compressBlock_lazy_generic, zstd/zstd.c:34232)
+    ZeLazy lz; lz.depth = depth; lz.attempts = 1u << (search_log < 6 ? search_log : 6u);
+    lz.mls = min_match < 4 ? 4u : (min_match > 6 ? 6u : min_match); lz.win = (u32)(win < (1ull << 31) ? win : (1ull << 31));
+    ZB_LAUNCH((zb_compress_blocks<false, ZE_UNIT, false, false, true>), n_ctas, ZE_THREADS, sizeof(ZeShared), st, src, jobs, n_jobs,
+              (ZeScratch*)scratch, slots, slot_bytes, outs, work_counter, dict, up, nullptr, lz);
 }
 
 // content-dictionary chains: the chunk indexes of a run, and its block jobs through the prefix mode
@@ -1599,7 +1748,7 @@ void zb_launch_compress_chain_blocks(const u8* src, const ZeBlockJob* jobs, u32 
     ZeDict dict; memset(&dict, 0, sizeof dict); dict.cct = segs;
     ZeUpload up; up.progress = nullptr; up.total = 0; up.status = nullptr;
     ZB_LAUNCH((zb_compress_blocks<false, ZE_UNIT, false, true>), n_ctas, ZE_THREADS, sizeof(ZeShared), st, src, jobs, n_jobs,
-              (ZeScratch*)scratch, slots, slot_bytes, outs, work_counter, dict, up, nullptr);
+              (ZeScratch*)scratch, slots, slot_bytes, outs, work_counter, dict, up, nullptr, ZeLazy{});
 }
 
 void zb_launch_frame_layout(const ZbSegment* segs, const ZeSegInfo* seginfo, const ZeBlockOut* outs, u32 n_segs, u32 checksum, u32 content_size,
